@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — Flash Checkpoint hot path on B200.
+"""bench.py — Flash Checkpoint hot path on H100.
 
 A "step" = one memory checkpoint of this rank's shard: the Llama-3-8B bf16
 state_dict (291 tensors, 16,060,522,496 bytes), resident in HBM, serialised
@@ -16,13 +16,14 @@ into the node's POSIX shared-memory segment in the reference's byte layout.
          descriptor table only (first step).
   stall_ms  what the training loop loses per checkpoint (the other half of
          BASELINE.json's metric): measured with a synthetic matmul step.
-  roofline  the gather (pack) kernel against the MEASURED copy bandwidth.
+  roofline  the gather (pack) kernel against the HBM bandwidth (MEASURED_PEAKS.json when
+         present, else the H100 SXM data sheet's 3.35 TB/s).
   cpu_baseline / --impl reference: the reference's memory save (per-tensor
          blocking device->pageable-shm copy_) on the same box and state_dict —
          the reference's own SharedMemoryHandler from oracle/_ref/pyref (kind
          "reference"), else the restatement oracle/ref_port.py (kind "port").
 
-Launch: python bench.py [--gpus N --steps K --warmup W] ; for N>1 under
+Launch: python bench.py [--gpus N --steps K --warmup W] [--dump-outputs DIR] ; for N>1 under
 torch.distributed.run, one rank per GPU, every rank saves its own 16 GB shard
 (weak scaling, no data-path collective).
 """
@@ -53,6 +54,8 @@ def parse():
     ap.add_argument("--scale", type=float, default=float(os.getenv("BENCH_SCALE", "1.0")),
                     help="shrink dim 0 of every 2-D tensor (debug only; 1.0 = BASELINE config)")
     ap.add_argument("--no-stall", action="store_true", help="skip the stall measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a fixed sample of the segment the last timed step wrote to DIR/*.npy")
     return ap.parse_args()
 
 
@@ -152,15 +155,26 @@ def measured_peak():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (of measured)"
     except Exception:
-        return 6650.0, "fallback 6.65 TB/s (of fallback)"
+        return 3350.0, "H100 SXM data sheet 3.35 TB/s (not measured)"
 
 
-def ncu_traffic():
-    p = os.path.join(ROOT, "profiles", "pack_kernel_ncu.json")
-    try:
-        return json.load(open(p)).get("dram_bytes_per_launch")
-    except Exception:
-        return None
+DUMP_ELEMENTS = 4 << 20
+
+
+def dump_outputs(out_dir, seg, nbytes):
+    """The bytes the last timed step left in the segment, read back as the bf16 values a
+    restoring caller receives: a fixed, seeded sample of DUMP_ELEMENTS of them as float32
+    (segment_bf16_sample.npy) and their element indices (segment_bf16_sample_index.npy).
+    The sample does not depend on the build, so two builds compare output for output."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    n = nbytes // 2
+    idx = np.unique(np.random.default_rng(0).integers(0, n, size=min(n, DUMP_ELEMENTS)))
+    bits = np.frombuffer(seg, dtype=np.uint16, count=n)[idx]
+    vals = (bits.astype(np.uint32) << 16).view(np.float32)
+    np.save(os.path.join(out_dir, "segment_bf16_sample.npy"), vals)
+    np.save(os.path.join(out_dir, "segment_bf16_sample_index.npy"), idx.astype(np.float64))
 
 
 # ---------------------------------------------------------------- reference arm --
@@ -322,7 +336,7 @@ def workload_config(S, world, scale):
         "payload_bytes_per_rank": S, "ranks": world,
         "sharding": "every rank saves its own full-size shard to its own segment "
                     "(DdpCheckpointer local_shard_num=world)",
-        "l2": "inputs (16 GB) and arena (16 GB) are far larger than the 126 MB L2; no flush needed",
+        "l2": "inputs (16 GB) and arena (16 GB) are far larger than the 50 MB L2; no flush needed",
     }
 
 
@@ -444,6 +458,7 @@ def run_ours(args):
     value = S * world * args.steps / raw_ms / 1e6
     pack_ms = sum(packs) / len(packs)
     drain_ms = sum(drains) / len(drains)
+    args.drain_ms = drain_ms
     peak, peak_src = measured_peak()
     achieved = 2 * S / pack_ms / 1e6
 
@@ -456,6 +471,8 @@ def run_ours(args):
         want = t.view(-1).view(torch.uint8)[:n].cpu().numpy()
         assert np.array_equal(img[off:off + n], want), "segment image mismatch"
     del img
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, seg, S)
     plan.destroy()
     ctx.host_unregister(addr)
     seg.close()
@@ -526,10 +543,8 @@ def run_ours(args):
         "fsdp": None,
         "roofline": {"bound": "hbm", "kernel": "fc_copy_tma<0> (gather/pack)",
                      "achieved": achieved, "peak": peak, "unit": "GB/s",
-                     "frac": achieved / peak, "traffic": ncu_traffic(),
-                     "traffic_source": "static: profiles/pack_kernel_ncu.json (one ncu --set "
-                                       "full capture of this kernel on this workload, "
-                                       "dram__bytes_read.sum + dram__bytes_write.sum)",
+                     "frac": achieved / peak, "traffic": None,
+                     "traffic_source": "not measured (no profiler capture of DRAM bytes)",
                      "algorithmic_bytes_per_launch": 2 * S, "avg_launch_ms": pack_ms,
                      "peak_source": peak_src},
         "drain": {"avg_ms": drain_ms, "GBps": S / drain_ms / 1e6, "bound": "PCIe Gen5 x16"},
@@ -755,7 +770,8 @@ def measure_cooperative(args, sd, S, world, dev):
            "ms_per_save": dt / args.steps * 1e3, "host_call_ms": sum(calls) / len(calls) * 1e3,
            "first_save_s": first, "slice_bytes": hi - lo,
            "pack_ms_slice": timings[0], "drain_ms_slice": timings[1],
-           "single_link_reference_policy_ms": S / 55.5e9 * 1e3,
+           # the raw leg's drain: the whole image over this rank's one PCIe link
+           "single_link_reference_policy_ms": getattr(args, "drain_ms", None),
            "image_matches_replicas": ok}
     drop_segment(ckpt.engine)
     return out
@@ -775,8 +791,15 @@ def measure_fsdp(args, world, rank, local, dev):
     from dlrover_b200.flash_checkpoint.fsdp_engine import FsdpCheckpointEngine
 
     mesh = init_device_mesh("cuda", (world,))
+    # the local shard (bf16 weights + two fp32 moments, 10 bytes per parameter) and its
+    # snapshot arena must fit in HBM together: 40 GB per rank at N=2 is 80 GB with the arena,
+    # more than an 80 GB H100 holds, so the shapes shrink until both take <= 80 % of it
+    full = shapes.scale_shapes(shapes.llama3_8b_shapes(), args.scale)
+    per_rank = sum(int(torch.Size(s).numel()) for _, s in full) * 10 / world
+    fit = 0.4 * torch.cuda.get_device_properties(dev).total_memory
+    fsdp_scale = min(1.0, fit / per_rank)
     factory = shapes.ShardedStateFactory(
-        shapes.scale_shapes(shapes.llama3_8b_shapes(), args.scale), world, rank, dev, mesh)
+        shapes.scale_shapes(full, fsdp_scale) if fsdp_scale < 1.0 else full, world, rank, dev, mesh)
     states = [factory.build(0), factory.build(1)]
     ckpt_dir = new_agent_namespace("f")
     engine = FsdpCheckpointEngine(ckpt_dir, PosixDiskStorage())
@@ -833,6 +856,7 @@ def measure_fsdp(args, world, rank, local, dev):
                    "one plan re-target, one gather kernel, one drain per rank), fresh tensors at "
                    "every save; value = bytes of all ranks / wall time (slowest rank)",
            "payload_bytes_per_rank": S_rank, "payload_bytes_total": total,
+           "shape_scale": fsdp_scale,
            "ms_per_save": dt / args.steps * 1e3,
            "host_call_ms": sum(calls) / len(calls) * 1e3,
            "host_call_ms_max": max(calls) * 1e3,
@@ -872,9 +896,16 @@ def measure_fresh_restore(ckpt, sd, S, ckpt_dir):
 
 
 def measure_stall(ckpt, sd, S, dev, world):
-    """Synthetic training loop: `inner` bf16 8192^3 matmuls per step on the
-    training stream.  Compare step time without checkpoints, with an async
-    memory checkpoint every `every` steps (ours), and with a blocking one."""
+    """Synthetic training loop: `inner` bf16 8192^3 matmuls per step on the training
+    stream.  Compares windows of `every` steps without a checkpoint, with an async memory
+    checkpoint (ours) and with a blocking one, the save issued after the window's first
+    step.  A power-limited card runs long matmul stretches at lower clocks than short
+    ones, so the three kinds of window are not timed in three long loops one after the
+    other: they alternate (base, async, base, blocking, ..., base) and every checkpoint
+    window is compared with the mean of the two base windows beside it.  Clocks and
+    throttle reasons are sampled during the windows."""
+    import statistics
+
     import torch
 
     from dlrover_b200.flash_checkpoint.api import StorageType
@@ -900,7 +931,7 @@ def measure_stall(ckpt, sd, S, dev, world):
         # the device by more than one step
         return float(c[0, 0].item())
 
-    # size the checkpoint interval so a drain (S over PCIe) always fits in it
+    # size the window so a drain (S over PCIe) always ends inside it
     for _ in range(3):
         train_step()
     torch.cuda.synchronize()
@@ -909,50 +940,72 @@ def measure_stall(ckpt, sd, S, dev, world):
         train_step()
     torch.cuda.synchronize()
     step_s = (time.perf_counter() - t0) / 5
-    drain_s = S / 45e9
+    drain_s = S / 40e9
     every = int(drain_s * 1.5 / step_s) + 2
 
-    def loop(save_mode):
-        # save_mode: None | "async" | "blocking"
+    def window(save_mode, step_id):
+        # save_mode: None | "async" | "blocking"; the wait for the drain after the
+        # window is not timed (it has ended inside the window unless the drain is slow)
         barrier_sync(world)
         t0 = time.perf_counter()
-        host_in_call, saves = 0.0, 0
-        for i in range(every * rounds):
+        host, saved = 0.0, False
+        for i in range(every):
             train_step()
-            if save_mode and i % every == every - 1:
+            if save_mode and i == 0:
                 before = ckpt.engine._cached_step
                 h0 = time.perf_counter()
-                ckpt.save_checkpoint(10_000 + i + (0 if save_mode == "async" else 100_000), sd,
-                                     storage_type=StorageType.MEMORY)
+                ckpt.save_checkpoint(step_id, sd, storage_type=StorageType.MEMORY)
                 if save_mode == "blocking":
                     ckpt.wait_memory_save()
-                host_in_call += time.perf_counter() - h0
-                saves += int(ckpt.engine._cached_step != before)
+                host = time.perf_counter() - h0
+                saved = ckpt.engine._cached_step != before
         torch.cuda.synchronize()
         dt = time.perf_counter() - t0
         ckpt.wait_memory_save()
-        return dt, host_in_call, saves
+        return save_mode, dt, host, saved
 
-    loop(None)
-    base = min(loop(None)[0], loop(None)[0])
-    asy, asy_host, n_a = loop("async")
-    blk, blk_host, n_b = loop("blocking")
+    window(None, 0)  # warm
+    clocks = ClockSampler(dev.index if dev.index is not None else 0)
+    clocks.start()
+    wins = []
+    for r in range(rounds):
+        wins.append(window(None, 0))
+        wins.append(window("async", 10_000 + 2 * r))
+        wins.append(window(None, 0))
+        wins.append(window("blocking", 10_001 + 2 * r))
+    wins.append(window(None, 0))
+    clk = clocks.stop()
+    stalls = {"async": [], "blocking": []}
+    host_async, saves = [], {"async": 0, "blocking": 0}
+    for k, (mode, dt, host, saved) in enumerate(wins):
+        if mode is None:
+            continue
+        base = (wins[k - 1][1] + wins[k + 1][1]) / 2
+        stalls[mode].append((dt - base) * 1e3)
+        saves[mode] += int(saved)
+        if mode == "async":
+            host_async.append(host * 1e3)
     timings = ckpt.engine.last_save_timings() or (None, None, None)
+    base_all = [w[1] for w in wins if w[0] is None]
     return {
-        "async": max((asy - base) / max(n_a, 1) * 1e3, 0.0),
-        "blocking": (blk - base) / max(n_b, 1) * 1e3,
-        "host_call_ms_async": asy_host / max(n_a, 1) * 1e3,
+        "async": statistics.median(stalls["async"]),
+        "blocking": statistics.median(stalls["blocking"]),
+        "async_per_window_ms": stalls["async"],
+        "blocking_per_window_ms": stalls["blocking"],
+        "host_call_ms_async": statistics.median(host_async),
         "pack_kernel_ms": timings[0],
-        "train_step_ms": base / (every * rounds) * 1e3,
+        "train_step_ms": statistics.median(base_all) / every * 1e3,
         "checkpoint_every_steps": every,
-        "saves_done": [n_a, n_b],
+        "saves_done": [saves["async"], saves["blocking"]],
         "saves_attempted": rounds,
-        "method": f"{every * rounds} synthetic steps of {inner} bf16 8192^3 matmuls + a "
-                  "loss.item()-style host read per step, a memory "
-                  f"checkpoint every {every} steps; stall = (loop wall time - wall time of the "
-                  "same loop without checkpoints) / #checkpoints; 'async' = product default "
-                  "(returns after enqueueing the gather kernel), 'blocking' = waits for the "
-                  "drain inside the step like the reference",
+        "clocks": clk,
+        "method": f"{rounds} rounds of 4 windows of {every} synthetic steps ({inner} bf16 8192^3 "
+                  "matmuls + a loss.item()-style host read per step): base, async checkpoint, "
+                  "base, blocking checkpoint, then a last base window; the save is issued after "
+                  "the window's first step; stall = window time - mean of the two base windows "
+                  "beside it, median over the rounds; 'async' = product default (returns after "
+                  "enqueueing the gather kernel), 'blocking' = waits for the drain inside the "
+                  "step like the reference",
     }
 
 

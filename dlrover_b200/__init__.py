@@ -1,4 +1,4 @@
-"""B200-native Flash Checkpoint (see DESIGN.md)."""
+"""H100-native Flash Checkpoint (see DESIGN.md)."""
 
 import os as _os
 

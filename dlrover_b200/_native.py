@@ -4,7 +4,7 @@ This is the only module that touches the shared library.  There is NO CPU
 fallback: if the library is missing or a call fails, ``NativeError`` is raised
 so a GPU box can never silently run the reference's per-tensor ``copy_`` loop
 (dlrover/python/elastic_agent/torch/ckpt_saver.py:198-231) instead of the
-sm_100a kernels.
+sm_90a kernels.
 """
 
 from __future__ import annotations
@@ -151,7 +151,7 @@ def load_library():
                 FC_EINVAL,
                 "load_library",
                 f"{_LIB_PATH} is not built; run __graft_entry__.build() "
-                "(nvcc -gencode arch=compute_100a,code=sm_100a). There is no CPU fallback.",
+                "(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU fallback.",
             )
         lib = ctypes.CDLL(_LIB_PATH, mode=ctypes.RTLD_LOCAL)
         for name, (restype, argtypes) in _SIGNATURES.items():
@@ -561,8 +561,8 @@ def get_context(device: int) -> Context:
             if not threads:
                 # first save / restart restore only; leave cores to the other local ranks
                 local_world = int(os.getenv("LOCAL_WORLD_SIZE", "1") or 1)
-                # 8 is the measured sweet spot (profiles/r02_staged_and_pin.md: more threads
-                # fault a fresh segment in more slowly and copy no faster)
+                # at most 8: more threads fault a fresh segment in more slowly and
+                # copy no faster
                 threads = max(2, min(8, (os.cpu_count() or 2) // max(1, 2 * local_world)))
             ctx.set_stage(threads, 0)
             _contexts[device] = ctx

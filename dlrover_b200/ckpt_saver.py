@@ -569,8 +569,7 @@ def _torch_save_writer():
         return torch.save
     from . import fast_torch_save
 
-    # measured on the B200 host (profiles/r01_fast_persist.md): 4 writers are the
-    # sweet spot for page-cache / tmpfs targets, more threads contend
+    # at most 4 writers: page-cache / tmpfs targets gain nothing from more, they contend
     threads = int(os.getenv("DLROVER_B200_PERSIST_THREADS", "0") or 0) or \
         max(1, min(4, (os.cpu_count() or 1) // 2))
     return lambda sd, path: fast_torch_save.save(sd, path, threads=threads)

@@ -21,8 +21,8 @@ the control segment (that is how a trainer recognises an agent that understands 
 with the reference's agent there is none and the trainer falls back to ``SharedDict``.
 
 Memory ordering: the header is written and read with plain stores / loads from Python
-(``struct.pack_into``); the seqlock is sound on hosts with total store order (x86-64: every
-B200 HGX host this was run on).  On a weakly ordered host (Grace) the odd/even sequence
+(``struct.pack_into``); the seqlock is sound on hosts with total store order (x86-64, the
+host CPU of HGX H100 systems).  On a weakly ordered host (Grace) the odd/even sequence
 stores need release / acquire fences — move ``publish`` / ``snapshot`` into the C library
 (``std::atomic_thread_fence``) before relying on it there.
 """

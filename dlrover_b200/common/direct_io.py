@@ -19,10 +19,9 @@ backed by a block device the payload can bypass the page cache:
     byte-identical (tests/test_direct_io.py compares sha256).
 
 `enabled_for(path)`: DLROVER_B200_DIRECT_IO=1 forces it (after a probe write), "auto" uses it on
-ext4 / xfs / btrfs / f2fs mounts, the default "0" leaves it off: on the GPU box of this project the
-checkpoint directory is an overlay file system, where O_DIRECT buys nothing (1.09 vs 1.08 GB/s
-including the final sync) and the buffered writer returns 3x sooner because 2 TB of page cache absorb
-the file (profiles/r02_persist.md) — how long the agent holds the shard lock is what matters there.
+ext4 / xfs / btrfs / f2fs mounts, the default "0" leaves it off: on an overlay file system O_DIRECT
+buys nothing and the buffered writer returns sooner while the page cache absorbs the file — how long
+the agent holds the shard lock is what matters there.
 """
 
 from __future__ import annotations

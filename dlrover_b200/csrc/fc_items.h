@@ -33,19 +33,16 @@ constexpr int kLsuThreads = 256;
 constexpr int kLsuUnroll = 4;
 constexpr uint32_t kDefaultChunk = 256u << 10;      // work-item size
 constexpr uint64_t kDmaPiece = 256ull << 20;        // restore fill memcpy size
-// Drain pacing.  Measured on B200 (tools/d2h_probe2.py, profiles/r01_d2h_pacing.md):
-// while a stream has ANOTHER D2H copy queued behind the one in flight, the
-// copy engine keeps serving that stream, and a small D2H copy from any other
-// stream of the process (a `loss.item()`!) starves until the whole checkpoint
-// has left the device (145-290 ms).  With exactly ONE piece in flight the
-// engine's queue empties for a moment after every piece and the foreign copy
+// Drain pacing (tools/d2h_probe2.py shows it): while a stream has ANOTHER D2H
+// copy queued behind the one in flight, the copy engine keeps serving that
+// stream, and a small D2H copy from any other stream of the process (a
+// `loss.item()`!) starves until the whole checkpoint has left the device.  With
+// exactly ONE piece in flight the engine's queue empties for a moment after every piece and the foreign copy
 // goes through after at most one piece.  The pump thread therefore submits piece
 // k+1 only after piece k completed.
-// Piece size (round 2, bench.py on one B200, profiles/r02_drain_modes.md): a
-// training loop with a `.item()` per step loses 9.2 ms per checkpoint with 32 MiB
-// pieces and 7.2 ms with 16 MiB pieces (each `.item()` issued during the 290 ms
-// drain waits for the piece in flight), for 55.1 vs 54.1 GB/s of checkpoint
-// throughput: the default favours the stall.  fc_set_drain /
+// Piece size: each `.item()` a training loop issues during the drain waits for
+// the piece in flight, so smaller pieces lose less of the step and a little
+// checkpoint throughput; the default favours the stall.  fc_set_drain /
 // DLROVER_B200_DRAIN_PIECE_MB change it.
 constexpr uint64_t kDrainPiece = 16ull << 20;
 constexpr int kDrainDepth = 1;

@@ -1,4 +1,4 @@
-// fc_kernels.cuh — the three copy kernels of the Flash Checkpoint path (sm_100a),
+// fc_kernels.cuh — the three copy kernels of the Flash Checkpoint path (sm_90a),
 // all templated on direction (0 = gather/pack: tensors -> arena, 1 = scatter):
 //   fc_copy_lsu        128-bit LDG/STG, any alignment (heads, tails, small ranges,
 //                      table slices of the windowed / hybrid saves)
@@ -63,8 +63,7 @@ __device__ __forceinline__ uint4 shfl_down1(const uint4& v) {
 // Output vector i needs the aligned words W[i] and W[i+1].  Every lane loads
 // its W[i] ONCE (coalesced 512 B per warp) and takes W[i+1] from its right
 // neighbour with a shuffle; only lane 31 loads the extra halo word.  (Loading
-// both words per lane re-fetched the shared sectors: ncu showed 18.7 GB of
-// DRAM reads for 16.06 GB of payload, profiles/r01_shifted_path.md.)
+// both words per lane fetches every straddled sector twice.)
 template <int Q>
 __device__ __forceinline__ void copy_shifted(const uint4* __restrict__ abase,
                                              uint4* __restrict__ dst, uint32_t nvec,
@@ -300,8 +299,8 @@ fc_copy_tma(const FcItem* __restrict__ items, uint32_t n_items, uint8_t* __restr
 // source span of each 16 KiB destination tile (+ one 16-B halo word) is
 // TMA-loaded into a shared-memory ring, 128 threads funnel-shift it from shared
 // to shared (two LDS.128 + four SHF + one STS.128 per 16 B), and the aligned
-// result is TMA-stored.  The LSU shifted path re-reads straddled sectors
-// (18.7 GB of DRAM reads for 16.06 GB, 5.98 ms); this one does not.
+// result is TMA-stored.  The LSU shifted path re-reads straddled sectors; this
+// one does not.
 constexpr int kShiftThreads = 256;
 // shared memory: in_stages x (tile + 128 B halo slot) input ring, 2 x tile
 // output double buffer, in_stages mbarriers

@@ -1,4 +1,4 @@
-// flashckpt.cu — device engine of the B200 Flash Checkpoint path (sm_100a only).
+// flashckpt.cu — device engine of the H100 Flash Checkpoint path (sm_90a only).
 //
 // What the reference does on this path (dlrover @ 468d632):
 //   ckpt_saver.py:198-231   per leaf: torch.frombuffer(shm).copy_(gpu_tensor)
@@ -24,8 +24,8 @@
 //   fc_copy_tma       one elected thread per CTA drives a ring of cp.async.bulk
 //                     global->shared (mbarrier complete_tx) and shared->global
 //                     (bulk_group) transfers: the 16-B congruent bodies.
-//                     Default 148 CTAs x 2 stages x 96 KiB: 4.76 ms for 32 GB of
-//                     traffic, 1.02x the measured copy peak.
+//                     Default: one CTA per SM (132 on H100 SXM) x 2 stages x
+//                     96 KiB, 192 KiB of the 227 KB of shared memory a block may use.
 //   fc_copy_tma_shift ranges whose source and destination are NOT congruent
 //                     mod 16: TMA in, funnel shift shared->shared, TMA out.
 //   fc_copy_lsu       256-thread CTAs, 128-bit LDG/STG, 4-way unrolled: heads,
@@ -94,14 +94,13 @@ extern "C" const char* fc_last_error(void) { return g_err; }
 
 struct fc_ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t copy_stream = nullptr;
   cudaStream_t copy_stream2 = nullptr;  // second leg of the ping-pong drain
   uint8_t* arena = nullptr;
   uint64_t arena_bytes = 0;
   uint64_t arena_cap = 0;  // 0 = unlimited; else fc_arena_reserve never allocates more
-  // tuning
-  // tuning: defaults picked from the B200 sweep in profiles/r01_sweep.md
+  // tuning (launch shapes of the three copy kernels)
   int variant = FC_VARIANT_TMA;
   int lsu_ctas_per_sm = 2;
   int tma_ctas_per_sm = 1;
@@ -504,12 +503,12 @@ extern "C" int fc_ctx_create(int device, fc_ctx** out) {
   for (cudaEvent_t* ev : evs)
     if (e == cudaSuccess) e = cudaEventCreate(ev);
   // The host-paced pump waits for piece k before it submits piece k+1, so its wake-up
-  // latency is on the critical path: a spinning wait gives 55.6 GB/s, a blocking one
-  // 52.4 GB/s at 32 MiB pieces (profiles/r01_d2h_pacing.md).  Spinning costs one busy
+  // latency is on the critical path: a spinning wait drains faster than a blocking one.
+  // Spinning costs one busy
   // host core while a checkpoint drains (~0.3 s) — nothing on a 128-core GPU host, a lot
   // in an 8-vCPU container.  Default: spin when the machine has more than 16 hardware
   // threads; otherwise sleep in a blocking wait AND chain the pieces on the device
-  // (ping-pong mode: no host round trip between pieces, profiles/r02_drain_modes.md).
+  // (ping-pong mode: no host round trip between pieces).
   // FC_DRAIN_SPIN=0/1 and FC_DRAIN_MODE=0/1 override.
   const char* spin_env = getenv("FC_DRAIN_SPIN");
   const bool many_cores = std::thread::hardware_concurrency() > 16;
@@ -675,7 +674,7 @@ static void mbind_preferred(uintptr_t lo, uintptr_t hi, int node) {
 // remote_per256 > 0: of every 256 consecutive 2-MiB blocks that many (spread evenly)
 // are bound to `remote` instead of `node` — when more GPUs of one socket drain at
 // once than its memory controllers absorb and the other socket is idle, a share of
-// the DMA writes goes over the inter-socket link (profiles/r02_numa_split.md).
+// the DMA writes goes over the inter-socket link.
 static void prefer_numa_node(void* host, uint64_t bytes, int node, int remote = -1,
                              int remote_per256 = 0) {
   if (node < 0) return;

@@ -15,7 +15,7 @@ Contract (reference @ 468d632, dlrover/python/elastic_agent/torch/ckpt_saver.py)
 
 What is different underneath: device-resident leaves are NOT copied one by one
 with blocking pageable cudaMemcpy (:221-231).  They are described once to
-libflashckpt (a cached plan), gathered by one sm_100a kernel into an HBM arena
+libflashckpt (a cached plan), gathered by one sm_90a kernel into an HBM arena
 on the caller's stream, and drained to the pinned segment by DMA on a side
 stream; `save_state_dict(..., blocking=False)` returns as soon as the kernel is
 enqueued and finishes the protocol from a completion thread.  Host-resident
@@ -418,7 +418,7 @@ def _numa_remote_share(device_index: int) -> int:
     """Of every 256 2-MiB blocks of the segment, how many to place on the OTHER socket.
     DLROVER_B200_NUMA_REMOTE_PER256 forces a value; "auto" derives it from how the local
     ranks' GPUs are spread over the two sockets (a ranks here, b there, a > b: (a-b)/(2a)
-    of this rank's pages go across) — see profiles/r02_numa_split.md for when it pays."""
+    of this rank's pages go across)."""
     env = os.getenv("DLROVER_B200_NUMA_REMOTE_PER256", "0").strip().lower()
     if env != "auto":
         try:

@@ -1,5 +1,5 @@
 /*
- * flashckpt.h — C-ABI of libflashckpt.so, the B200 (sm_100a) device engine that
+ * flashckpt.h — C-ABI of libflashckpt.so, the H100 (sm_90a) device engine that
  * sits UNDER the Flash Checkpoint shared-memory handler.
  *
  * The reference (dlrover @ 468d632) has no native boundary on this path: the
@@ -52,7 +52,7 @@ enum {
 
 /* kernel variants (fc_set_variant / fc_pack_async 'variant' argument) */
 enum {
-  FC_VARIANT_AUTO = 0, /* library default (the faster one as measured on B200) */
+  FC_VARIANT_AUTO = 0, /* library default (FC_VARIANT_TMA) */
   FC_VARIANT_LSU = 1,  /* 128-bit LDG/STG register path for everything         */
   FC_VARIANT_TMA = 2   /* cp.async.bulk global->smem->global ring for the 16-B
                           congruent bodies + LSU kernel for heads/tails/shifted */
@@ -257,7 +257,7 @@ int fc_set_drain(fc_ctx* ctx, uint64_t piece_bytes, int depth);
  *                        the DEVICE for piece k-1: no stream ever has a second copy
  *                        queued, no host round trip between pieces, the host thread
  *                        sleeps in a blocking wait.  Small pieces then cost no
- *                        throughput (profiles/r02_drain_modes.md). */
+ *                        throughput. */
 enum { FC_DRAIN_HOST_PACED = 0, FC_DRAIN_PINGPONG = 1 };
 int fc_set_drain_mode(fc_ctx* ctx, int mode);
 

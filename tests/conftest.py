@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "timeout: per-test timeout (pytest-timeout)")
     # The suite states what the DEFAULT configuration does (several tests assert that a
     # feature is on): switches left in the caller's shell must not change the outcome.

@@ -1,6 +1,6 @@
-"""One rank of the multi-rank parity cases (launched by tests/test_multi_gpu.py and by
-tools/gpu_call_*.sh under torch.distributed.run).  NCCL + CUDA on the GPU box; the same
-cases run with `--backend gloo --device cpu` here, so the host logic is covered without a GPU.
+"""One rank of the multi-rank parity cases (launched by tests/test_multi_gpu.py under
+torch.distributed.run).  NCCL + CUDA on GPUs; the same cases run with `--backend gloo
+--device cpu`, so the host logic is covered without a GPU.
 
 Every case ends with EVERY rank comparing its whole segment byte-for-byte with the oracle
 image (oracle/shm_layout.py) of what that rank handed to the engine, and restoring it.

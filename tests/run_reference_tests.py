@@ -1,23 +1,27 @@
 """Run the REFERENCE's own hot-path unit tests against THIS implementation.
 
-The reference checkout (/root/reference) supplies the test files and their
-helpers (local master, fixtures); the flash-checkpoint modules they import —
+The reference's package, byte-compiled by oracle/build_ref.py into oracle/_ref/reftests,
+supplies the test modules and their helpers (local master, fixtures); the
+flash-checkpoint modules they import —
 dlrover.python.common.{multi_process,storage,...},
 dlrover.python.elastic_agent.torch.ckpt_saver,
 dlrover.trainer.torch.flash_checkpoint.* — are replaced by this package's
-modules before collection (dlrover_b200.compat.ALIASES, real parent packages
-kept).  Usage (build container only):
+modules before the tests are loaded (dlrover_b200.compat.ALIASES, real parent
+packages kept).  The modules are sourceless, so unittest (all of them are
+unittest.TestCase suites) runs them, not pytest.  Usage:
 
-    python tests/run_reference_tests.py [pytest args...]
+    python tests/run_reference_tests.py [test module or reference-relative path ...]
 """
 
 import importlib
 import os
 import sys
+import tempfile
+import unittest
 from unittest import mock
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = os.path.join(ROOT, "oracle", "_ref", "reftests")
 
 DEFAULT_FILES = [
     "dlrover/python/tests/test_multi_process.py",
@@ -82,21 +86,26 @@ def install_overrides():
 
 
 if __name__ == "__main__":
-    import pytest
-
     # children started by the tests (mp.spawn) get the overrides through
     # tests/_ref_site/sitecustomize.py
     os.environ["DLROVER_B200_REF_TESTS"] = "1"
+    # the reference's event exporter logs to /tmp/dlrover by default, a directory that may
+    # belong to another user: every run gets its own (inherited by spawned children)
+    work = tempfile.mkdtemp(prefix="fc_reftests_")
+    os.environ["DLROVER_EVENT_FILE_DIR"] = os.path.join(work, "events")
     site = os.path.join(ROOT, "tests", "_ref_site")
     os.environ["PYTHONPATH"] = os.pathsep.join(
         [site, ROOT, REF] + [p for p in os.environ.get("PYTHONPATH", "").split(os.pathsep) if p])
     sys._fc_ref_overrides = True
     swapped = install_overrides()
     print(f"[run_reference_tests] {len(swapped)} reference modules replaced by dlrover_b200")
-    args = sys.argv[1:]
-    files = [a for a in args if a.endswith(".py")]
-    opts = [a for a in args if not a.endswith(".py")]
-    if not files:
-        files = DEFAULT_FILES
-    os.chdir(REF)
-    sys.exit(pytest.main(["-q", "-p", "no:cacheprovider", "--rootdir", REF] + opts + files))
+    names = [a[:-3].replace("/", ".") if a.endswith(".py") else a
+             for a in (sys.argv[1:] or DEFAULT_FILES)]
+    os.chdir(work)
+    suite = unittest.defaultTestLoader.loadTestsFromNames(names)
+    result = unittest.TextTestRunner(verbosity=2).run(suite)
+    failed = len(result.failures) + len(result.errors) + len(result.unexpectedSuccesses)
+    passed = result.testsRun - failed - len(result.skipped) - len(result.expectedFailures)
+    print(f"{passed} passed" + (f", {failed} failed" if failed else "")
+          + (f", {len(result.skipped)} skipped" if result.skipped else ""), flush=True)
+    sys.exit(0 if failed == 0 else 1)

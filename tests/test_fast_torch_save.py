@@ -1,7 +1,6 @@
 """fast_torch_save.fast_save must produce EXACTLY the bytes of torch.save
 (the agent's persist format, reference ckpt_saver.py:1079-1122).  The >4 GiB
-zip64 cases (offsets past 4 GiB, one tensor >= 4 GiB) were verified byte-for-
-byte in the build container (profiles/r01_fast_persist.md); they run here only
+zip64 cases (offsets past 4 GiB, one tensor >= 4 GiB) run only
 with FC_SLOW_TESTS=1 because each needs ~10 GB of RAM and ~40 s."""
 
 import hashlib

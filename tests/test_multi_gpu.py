@@ -3,9 +3,9 @@
   * on CPU (not gpu-marked): world_size 2 over gloo, every case — the host logic of the
     N>1 paths (DCP planning + plan reuse, per-rank segments, cooperative slices, control
     segment handshake, topology stand-ins);
-  * on the GPU box (gpu-marked): NCCL, one rank per GPU, 2 ranks and — when the box has
-    them — 8 ranks.  A box with a single GPU skips these (NCCL refuses two ranks on one
-    device); the 2- and 8-GPU runs of this round are committed under profiles/.
+  * on GPUs (gpu-marked): NCCL, one rank per GPU, 2 ranks and — when the machine has
+    them — 8 ranks.  A machine with a single GPU skips these (NCCL refuses two ranks on
+    one device).
 
 Every rank compares its whole segment byte-for-byte with the oracle image of what it
 handed to the engine and restores it (see the worker's docstring)."""
@@ -85,8 +85,7 @@ def _gpus():
 @pytest.mark.parametrize("case", CASES + ["fsdp_full"])
 def test_nccl_ranks_on_gpus(case, world):
     if _gpus() < world:
-        pytest.skip(f"needs {world} GPUs on one box, this one has {_gpus()} "
-                    "(see profiles/r02_multi_gpu_tests.md for the runs of this round)")
+        pytest.skip(f"needs {world} GPUs on one machine, this one has {_gpus()}")
     extra = ("--scale", str(1 / 32), "--flat-mib", "256")
     if case == "zero3":
         extra += ("--in-place", "--snapshot-mib", "300")

@@ -1,10 +1,10 @@
 """Interoperability with the REFERENCE's agent half: the reference's own
-AsyncCheckpointSaver (imported from /root/reference in a separate process, as
-`dlrover-run` would host it) serves OUR trainer-side DdpCheckpointer running in
-wire-compat mode: lock / queue / dict RPCs, the meta tree, the saver ClassMeta
-and the SAVE event all cross the process boundary as the reference's pickles,
-and the reference persists our shared-memory bytes with its own code.
-Runs only where /root/reference exists (the build container)."""
+AsyncCheckpointSaver (its byte code under oracle/_ref/pyref, built by oracle/build_ref.py,
+run in a separate process, as `dlrover-run` would host it) serves OUR trainer-side
+DdpCheckpointer running in wire-compat mode: lock / queue / dict RPCs, the meta tree, the
+saver ClassMeta and the SAVE event all cross the process boundary as the reference's
+pickles, and the reference persists our shared-memory bytes with its own code.
+Runs only where oracle/_ref/pyref has been built."""
 
 import os
 import subprocess
@@ -15,11 +15,17 @@ import uuid
 import pytest
 import torch
 
-REF = "/root/reference"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+REF = os.path.join(ROOT, "oracle", "_ref", "pyref")
 
-pytestmark = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "dlrover")),
-                                reason="needs the reference checkout")
+
+def _ref_trainer_built():
+    return os.path.exists(os.path.join(REF, "dlrover", "trainer", "torch", "flash_checkpoint",
+                                       "ddp.pyc"))
+
+
+pytestmark = pytest.mark.skipif(not _ref_trainer_built(),
+                                reason="oracle/_ref/pyref not built (no reference to build it from)")
 
 AGENT = r"""
 import sys, time

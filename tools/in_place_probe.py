@@ -1,5 +1,6 @@
 """Exposed stall of a checkpoint whose state does not fit in HBM twice: Llama-3-8B bf16
-weights + AdamW fp32 moments (80.3 GB at PROBE_SCALE=1) on one B200, with a ballast
+weights + AdamW fp32 moments (80.3 GB at PROBE_SCALE=1, 40 GB at the default 0.5, which
+leaves an 80 GB H100 room for the synthetic step) on one GPU, with a ballast
 tensor standing in for activations so that a snapshot arena cannot be allocated.
 
 Modes (one process each, PROBE_MODE):
@@ -30,7 +31,7 @@ import torch
 from dlrover_b200 import shapes
 from dlrover_b200.flash_checkpoint.api import DdpCheckpointer, StorageType
 
-scale = float(os.getenv("PROBE_SCALE", "1.0"))
+scale = float(os.getenv("PROBE_SCALE", "0.5"))
 step_ms = float(os.getenv("PROBE_STEP_MS", "400"))
 every = int(os.getenv("PROBE_EVERY", "4"))
 rounds = int(os.getenv("PROBE_ROUNDS", "3"))

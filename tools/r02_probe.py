@@ -1,4 +1,5 @@
-"""Round-2 measurements on one B200 (writes JSON lines to gpurun_out/r02_probe.jsonl):
+"""Drain, pinning and hybrid-snapshot measurements on one GPU (prints JSON lines and appends
+them to $PROBE_OUT_DIR/r02_probe.jsonl, by default under the system's temporary directory):
 
   drain     pacing modes x piece sizes: drain GB/s and the latency a foreign `.item()`
             sees while the checkpoint drains (host-paced depth-1 vs two-stream ping-pong)
@@ -15,6 +16,7 @@ import mmap
 import os
 import statistics
 import sys
+import tempfile
 import threading
 import time
 
@@ -25,7 +27,7 @@ import torch  # noqa: E402
 from dlrover_b200 import _native as native  # noqa: E402
 from dlrover_b200 import shapes  # noqa: E402
 
-OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
+OUT = os.environ.get("PROBE_OUT_DIR") or os.path.join(tempfile.gettempdir(), "fc_probe")
 os.makedirs(OUT, exist_ok=True)
 LOG = open(os.path.join(OUT, "r02_probe.jsonl"), "a")
 
