@@ -27,6 +27,7 @@ from __future__ import annotations
 
 import copy
 import os
+import threading
 import time
 from abc import ABCMeta, abstractmethod
 from datetime import timedelta
@@ -133,6 +134,22 @@ def verify_all_rank_step_consistent(group: Optional[dist.ProcessGroup], step):
         dist.all_gather(everyone, mine, group=group)
         values = [float(t.item()) for t in everyone]
     return all(v == values[0] for v in values)
+
+
+class ShardLockClaim:
+    """The shard lock as one save holds it (`acquired`: the save took it).  Whichever way
+    the save ends first (skipped, completed, failed drain, exception) gives it back;
+    release() releases at most once, so the paths need not know about each other."""
+
+    def __init__(self, lock: SharedLock, acquired: bool):
+        self._lock = lock if acquired else None
+        self._mutex = threading.Lock()
+
+    def release(self):
+        with self._mutex:
+            lock, self._lock = self._lock, None
+        if lock is not None:
+            lock.release()
 
 
 def timer(func):
@@ -530,6 +547,7 @@ class CheckpointEngine(metaclass=ABCMeta):
 
         # ---- leader ----
         acquired = bool(self._shm_lock.acquire(blocking)) if ready else False
+        claim = ShardLockClaim(self._shm_lock, acquired)
         try:
             join = patience if self._coop_established else float(
                 os.getenv("DLROVER_B200_COOP_JOIN_TIMEOUT_S", "5"))
@@ -541,8 +559,7 @@ class CheckpointEngine(metaclass=ABCMeta):
                     "reference does.")
                 ctl.next_coop_seq(aborted=True)
                 self._coop_wanted = False
-                if acquired:
-                    self._shm_lock.release()
+                claim.release()
                 return self._SOLO
             node_ready = acquired and followers_ready
             all_ready = node_ready
@@ -555,37 +572,28 @@ class CheckpointEngine(metaclass=ABCMeta):
                 logger.info(f"Rank {self._rank} skips the cooperative save of step {conf.step}: "
                             "not every rank is ready (the agent is persisting, or a drain is "
                             "in flight).")
-                if acquired:
-                    self._shm_lock.release()
+                claim.release()
                 return False
             state_dict[DLROVER_CKPT_CONFIG_KEY] = conf
             coop = CoopContext(ctl, 0, local_world, seq - 1, timeout=float(self._save_timeout))
-
-            def completed():
-                if acquired:
-                    self._shm_lock.release()
-
-            def failed():
-                # torn segment: writing_shm stays set; only the lock goes back
-                if acquired:
-                    self._shm_lock.release()
-
             # the handler opens save `seq` once the segment has its size and the
-            # announcement is out
+            # announcement is out; a failed drain leaves writing_shm set (torn segment)
+            # and only gives the lock back
             if shards:
                 handler.save_shards_as_full(state_dict, coop,
                                             blocking=not self._async_drain or blocking,
-                                            stream=self.snapshot_stream, on_complete=completed,
-                                            on_error=failed)
+                                            stream=self.snapshot_stream,
+                                            on_complete=claim.release, on_error=claim.release)
             else:
                 handler.save_state_dict(state_dict, blocking=not self._async_drain or blocking,
-                                        on_complete=completed, on_error=failed,
+                                        on_complete=claim.release, on_error=claim.release,
                                         stream=self.snapshot_stream, coop=coop)
         except BaseException:
             if ctl.coop_seq() < seq:
                 ctl.next_coop_seq(aborted=True)  # wherever it failed: nobody is left waiting
-            if acquired and handler.pending_save() is None and self._shm_lock.locked():
-                self._shm_lock.release()
+            # the handler queues a drain as the last step of a save: one that raised has
+            # queued none, and a blocking drain that failed has run on_error already
+            claim.release()
             raise
         self._coop_established = True
         self._cached_step = conf.step
@@ -683,6 +691,7 @@ class CheckpointEngine(metaclass=ABCMeta):
         # While our own drain runs we still hold the lock: report "not acquired"
         # without bothering the agent.
         acquired = False if pending is not None else self._shm_lock.acquire(blocking)
+        claim = ShardLockClaim(self._shm_lock, acquired)
         logger.info(f"{self._rank}-{self._local_rank} acquired the lock of shared memory: "
                     f"{acquired} for step: {conf.step}.")
         all_rank_ready = check_all_rank_ready(self._saver_group, acquired)
@@ -691,32 +700,26 @@ class CheckpointEngine(metaclass=ABCMeta):
             logger.info(f"Rank {self._rank} skips the save the checkpoint in CPU memory since "
                         "it is saving the latest checkpoint from the CPU memory into the "
                         "storage.")
-            if acquired:
-                self._shm_lock.release()
+            claim.release()
             return False
         state_dict[DLROVER_CKPT_CONFIG_KEY] = conf
 
         def completed():
-            if acquired:
-                self._shm_lock.release()
+            claim.release()
             self._replica_manager.backup(self._shm_handler)
 
         try:
             # replica backup issues collectives: keep those on the calling thread
             sync = not self._async_drain or self._replica_manager.has_replica()
-            def failed():
-                # the segment is torn (writing_shm stays set): give the lock back so
-                # later saves are attempted instead of being skipped forever
-                if acquired:
-                    self._shm_lock.release()
-
+            # a failed drain leaves the segment torn (writing_shm stays set): the lock
+            # goes back so later saves are attempted instead of being skipped forever
             self._shm_handler.save_state_dict(state_dict, blocking=sync, on_complete=completed,
-                                              on_error=failed, stream=self.snapshot_stream)
+                                              on_error=claim.release,
+                                              stream=self.snapshot_stream)
         except BaseException:
-            # raised before a completion thread took over (the blocking path runs
-            # `failed` itself)
-            if acquired and self._shm_handler.pending_save() is None and self._shm_lock.locked():
-                self._shm_lock.release()
+            # the handler queues a drain as the last step of a save: one that raised has
+            # queued none, and a blocking drain that failed has run on_error already
+            claim.release()
             raise
         self._cached_step = conf.step
         return True

@@ -62,6 +62,7 @@ from ..common.constants import CheckpointConstant
 from ..common.log import default_logger as logger
 from .engine import (
     CheckpointEngine,
+    ShardLockClaim,
     all_reduce_flags,
     check_all_rank_ready,
     timer,
@@ -329,9 +330,9 @@ class SharedMemoryWriter(StorageWriter):
     """DCP StorageWriter whose storage is the shared-memory segment.
 
     Beyond the reference's writer (fsdp_engine.py:158-232):
-      * `announce` (set by the engine) publishes "segment is being written" — inline when
-        host tensors are among the items, else from the completion thread with the drain
-        held until it is out (see SharedMemoryHandler.write_ranges);
+      * `announce` (set by the engine) publishes "segment is being written" before the
+        first byte of the segment changes (SharedMemoryHandler.write_ranges decides
+        whether inline or from the completion thread with the drain held);
       * the non-sharded objects of the LOCAL plan (before torch dedups replicated entries
         over the ranks) are kept per rank: replicated means every rank has them, so no
         rank needs another rank's copy to restore from its own memory
@@ -354,7 +355,6 @@ class SharedMemoryWriter(StorageWriter):
         self.no_shard: Optional[_DeferredHostCopy] = None
         self.announce = None   # Callable[[], None] or None
         self.on_error = None
-        self.announced_inline = False
 
     def reset(self, checkpoint_id: Union[str, os.PathLike, None] = None) -> None:
         pass
@@ -390,20 +390,13 @@ class SharedMemoryWriter(StorageWriter):
                 objects[item.index.fqn] = data.detach() if torch.is_tensor(data) else data
         self.no_shard = _DeferredHostCopy(objects)
         self.pending = None
-        self.announced_inline = False
-        announce = self.announce
         if total > 0:
             self.shm_handler.ensure_segment(total)
-            deferred = announce is not None and not self.blocking and bool(dev) and not host
-            if announce is not None and not deferred:
-                announce()
-                self.announced_inline = True
             self.pending = self.shm_handler.write_ranges(
                 dev, host, raw, blocking=self.blocking, keepalive=[d for d, _, _ in dev],
-                pre_drain=announce if deferred else None, on_error=self.on_error)
-        elif announce is not None:
-            announce()
-            self.announced_inline = True
+                announce=self.announce, on_error=self.on_error)
+        elif self.announce is not None:
+            self.announce()
         self.last_results = results
         self.metadata["no_shard_data"] = objects  # (reference attribute; host copies: no_shard.get())
         fut: Future[List[WriteResult]] = Future()
@@ -650,7 +643,6 @@ class FsdpCheckpointEngine(CheckpointEngine):
         self._shm_reader = SharedMemoryReader(self._shm_handler)
         self._plan_cache: Optional[Dict[str, Any]] = None
         self._published_meta: Dict[str, Any] = {}
-        self._meta_tree_published = False
         self.last_save_reused_plan = False
 
     def get_saving_ranks(self):
@@ -705,6 +697,7 @@ class FsdpCheckpointEngine(CheckpointEngine):
         handler, writer = self._shm_handler, self._shm_writer
         pending = handler.pending_save()
         acquired = False if pending is not None else bool(self._shm_lock.acquire(blocking=False))
+        claim = ShardLockClaim(self._shm_lock, acquired)
         planner = _save_planner()
         changed = True
         try:
@@ -723,13 +716,11 @@ class FsdpCheckpointEngine(CheckpointEngine):
             logger.info(f"Rank {self._rank} skips the save the checkpoint in CPU memory since "
                         "it is saving the latest checkpoint from the CPU memory into the "
                         "storage.")
-            if acquired:
-                self._shm_lock.release()
+            claim.release()
             return False
 
         conf = CheckpointConfig(rank=self._rank, group_rank=self._group_rank,
                                 world_size=self._world_size, step=step)
-        conf.writing_shm = True
         name = CheckpointConstant.MODEL_STATES_NAME
         reuse = n_changed == 0
         previous = dict(self._published_meta)  # what the agent holds for this shard now
@@ -741,20 +732,15 @@ class FsdpCheckpointEngine(CheckpointEngine):
             if reuse:
                 meta = {DLROVER_CKPT_CONFIG_KEY: conf, "dcp_metadata": cache["dcp_metadata"],
                         "no_shard_data": writer.no_shard.get()}
-                handler.metadata.next_unchanged = self._meta_tree_published
             else:
                 meta = {**previous, DLROVER_CKPT_CONFIG_KEY: conf}
-                handler.metadata.next_unchanged = bool(previous) and self._meta_tree_published
-            handler.metadata.payload_bytes = handler._buffer_size
-            handler.metadata.set(meta)
+            # the meta plane holds the last save's tree (`previous`; under a reused plan
+            # the same tree) if that save's final publication went through
+            handler._set_meta(meta, True, handler._meta_published, handler._buffer_size)
 
-        def failed():
-            # the segment is torn: the meta keeps writing_shm=True (the agent and a
-            # restarted trainer refuse it); only the lock goes back so later saves run
-            if acquired:
-                self._shm_lock.release()
-
-        writer.announce, writer.on_error = announce, failed
+        # a failed drain leaves the segment torn: the meta keeps writing_shm=True (the
+        # agent and a restarted trainer refuse it); only the lock goes back so later saves run
+        writer.announce, writer.on_error = announce, claim.release
         try:
             conf.paths = {name: os.path.join(paths[name], f"__{self._rank}_0{DEFAULT_SUFFIX}")}
             if reuse:
@@ -783,40 +769,33 @@ class FsdpCheckpointEngine(CheckpointEngine):
             conf.paths = {name: os.path.join(paths[name], writer.file_name)}
         except BaseException:
             writer.announce = writer.on_error = None
-            if acquired:
-                try:
-                    handler.wait_pending()
-                except BaseException:
-                    pass
-                if self._shm_lock.locked():
-                    self._shm_lock.release()
+            # a drain that write_data queued may still read the tensors, and its
+            # completion publishes nothing: the lock goes back once it is over
+            try:
+                handler.wait_pending()
+            except BaseException:
+                pass
+            claim.release()
             raise
         writer.announce = writer.on_error = None
         self.last_save_reused_plan = reuse
         no_shard = writer.no_shard
 
         def completed():
-            conf.writing_shm = False
-            meta = {DLROVER_CKPT_CONFIG_KEY: conf, "dcp_metadata": dcp_metadata,
-                    "no_shard_data": no_shard.get()}
-            # only the header flips when the announcement already carried this tree
-            handler.metadata.next_unchanged = reuse and self._meta_tree_published
-            handler.metadata.payload_bytes = handler._buffer_size
-            handler.metadata.set(meta)
-            self._published_meta = {"dcp_metadata": dcp_metadata,
-                                    "no_shard_data": meta["no_shard_data"]}
-            self._meta_tree_published = True
-            if acquired:
-                self._shm_lock.release()
+            try:
+                meta = {DLROVER_CKPT_CONFIG_KEY: conf, "dcp_metadata": dcp_metadata,
+                        "no_shard_data": no_shard.get()}
+                # only the header flips when the announcement already carried this tree
+                handler._set_meta(meta, False, reuse, handler._buffer_size)
+                self._published_meta = {"dcp_metadata": dcp_metadata,
+                                        "no_shard_data": meta["no_shard_data"]}
+            finally:
+                claim.release()
 
         drain = writer.pending
         if drain is None or drain.done():
-            try:
-                if drain is not None:
-                    drain.wait()  # re-raises a drain error
-            except BaseException:
-                failed()
-                raise
+            if drain is not None:
+                drain.wait()  # re-raises a drain error (its on_error gave the lock back)
             completed()
         else:
             import threading
@@ -826,12 +805,11 @@ class FsdpCheckpointEngine(CheckpointEngine):
                     drain.wait()
                 except BaseException as e:
                     logger.error(f"FSDP shard drain of step {conf.step} failed: {e}")
-                    return  # write_ranges' on_error (= failed) already ran
+                    return  # write_ranges' on_error gave the lock back
                 try:
                     completed()
                 except BaseException as e:
                     logger.error(f"publishing step {conf.step} failed: {e}", exc_info=True)
-                    failed()
 
             t = threading.Thread(target=waiter, name="fc-fsdp-drain", daemon=True)
             t.start()

@@ -134,8 +134,7 @@ class _Layout:
     """Result of one planning walk over a state_dict."""
 
     __slots__ = ("meta", "total", "device_leaves", "host_leaves", "leaf_metas", "reused",
-                 "extras", "shape_hash", "unchanged", "dev_ptrs", "dev_dense", "dev_offs",
-                 "dev_lens")
+                 "extras", "shape_hash", "unchanged")
 
     def __init__(self):
         self.meta: Any = None
@@ -147,11 +146,6 @@ class _Layout:
         self.extras: list = []  # non-tensor leaves, traversal order
         self.shape_hash = 0     # hash over the keys / container kinds met by the walk
         self.unchanged = False  # same meta tree as `prev` (keys, TensorMetas, extras)
-        # device leaves as the native layer wants them, gathered by the same walk
-        self.dev_ptrs: List[int] = []
-        self.dev_dense = True
-        self.dev_offs: List[int] = []
-        self.dev_lens: List[int] = []
 
 
 _IMMUTABLE_LEAVES = frozenset({int, float, str, bool, bytes, type(None), complex, torch.dtype,
@@ -174,7 +168,6 @@ def plan_layout(state_dict, prev: Optional["_Layout"] = None) -> _Layout:
     reused = 0
     shape_hash = 0
     extras = lay.extras
-    dev_ptrs, dev_offs, dev_lens = lay.dev_ptrs, lay.dev_offs, lay.dev_lens
 
     def walk(value):
         nonlocal total, reused, shape_hash
@@ -191,15 +184,7 @@ def plan_layout(state_dict, prev: Optional["_Layout"] = None) -> _Layout:
             metas.append(m)
             nbytes = m.numel * m.element_size
             if nbytes:
-                if value.is_cuda:
-                    dev.append((value, m))
-                    dev_ptrs.append(value.data_ptr())
-                    dev_offs.append(total)
-                    dev_lens.append(nbytes)
-                    if not value.is_contiguous():
-                        lay.dev_dense = False
-                else:
-                    host.append((value, m))
+                (dev if value.is_cuda else host).append((value, m))
                 total += nbytes
             return m
         kind = type(value)
@@ -479,27 +464,6 @@ def _triples(leaves):
     return [(t, m.offset, m.numel * m.element_size) for t, m in leaves]
 
 
-class _LeafRanges:
-    """(tensor, offset, nbytes) triples of a layout's device leaves, built only if
-    somebody iterates them (the common save already has the ptr/offset/length lists)."""
-
-    def __init__(self, leaves):
-        self._leaves = leaves
-
-    def __bool__(self):
-        return bool(self._leaves)
-
-    def __len__(self):
-        return len(self._leaves)
-
-    def __iter__(self):
-        return iter(_triples(self._leaves))
-
-    def __getitem__(self, i):
-        t, m = self._leaves[i]
-        return (t, m.offset, m.numel * m.element_size)
-
-
 def _clip_triples(triples, lo: int, hi: int):
     """(tensor, segment offset, nbytes) triples cut to segment bytes [lo, hi): the part of
     a tensor that falls inside becomes a uint8 view on its bytes."""
@@ -711,14 +675,14 @@ class PendingSave:
     """Handle of a save whose drain is still running on the copy stream."""
 
     def __init__(self, ctx: Optional[native.Context], ticket: int, finish: Callable[[], None],
-                 keepalive: list, pre_drain: Optional[Callable[[], None]] = None,
+                 keepalive: list, announce: Optional[Callable[[], None]] = None,
                  on_error: Optional[Callable[[], None]] = None):
         self._on_error = on_error
         self._ctx = ctx
         self._ticket = ticket
         self._finish = finish
         self._keepalive = keepalive
-        self._pre_drain = pre_drain  # set <=> the drain is held until we release it
+        self._announce = announce  # set <=> the drain is held until it has run
         self._done = threading.Event()
         self._error: Optional[BaseException] = None
         self._lock = threading.Lock()
@@ -730,9 +694,9 @@ class PendingSave:
             if self._done.is_set():
                 return
             try:
-                if self._pre_drain is not None:
+                if self._announce is not None:
                     try:
-                        self._pre_drain()  # e.g. publish writing_shm=True to the agent
+                        self._announce()  # writing_shm=True to the agent, then raw chunks
                     except BaseException:
                         # the agent does not know the segment is about to change: leave
                         # every byte of it alone (the previous checkpoint stays valid)
@@ -1056,11 +1020,6 @@ class SharedMemoryHandler:
             self._stager = _DeviceStager(index)
         return self._stager
 
-    def _stager_for_ranges(self, device_ranges) -> _DeviceStager:
-        if isinstance(device_ranges, _LeafRanges):
-            return self._stager_for([t for t, _ in device_ranges._leaves])
-        return self._stager_for([r[0] for r in device_ranges])
-
     def ensure_segment(self, total: int):
         """Map a segment of exactly `total` bytes (re-creating it on a size
         change)."""
@@ -1078,11 +1037,10 @@ class SharedMemoryHandler:
     def write_ranges(self, device_ranges, host_ranges, raw_chunks=(), *, blocking=True,
                      stream=None, finish: Optional[Callable[[], None]] = None,
                      keepalive: Optional[list] = None,
-                     pre_drain: Optional[Callable[[], None]] = None,
+                     announce: Optional[Callable[[], None]] = None,
                      on_error: Optional[Callable[[], None]] = None,
                      in_place: Optional[bool] = None,
-                     window: Optional[Tuple[int, int]] = None, compact: bool = False,
-                     prepared_hint=None):
+                     window: Optional[Tuple[int, int]] = None, compact: bool = False):
         """Move bytes into the (already sized) segment.
 
         device_ranges / host_ranges: (tensor, segment offset, nbytes) for CUDA /
@@ -1090,6 +1048,8 @@ class SharedMemoryHandler:
         one gather kernel + DMA drain, the rest is written by the host right
         away.  `finish` runs once everything has landed — inline when blocking,
         else on the completion thread of the returned PendingSave.
+        announce: publishes writing_shm=True; it runs before the first byte of the
+        segment changes, inline or, with the drain held, on the completion thread.
         in_place (default: self.in_place): no snapshot — the drain reads the CUDA
         tensors themselves, so they must not be written until the save is done
         (wait_pending / PendingSave.wait).  Also chosen, together with blocking,
@@ -1103,24 +1063,28 @@ class SharedMemoryHandler:
         """
         keepalive = keepalive if keepalive is not None else []
 
-        def write_raw():
+        def announce_then_raw():
+            if announce is not None:
+                announce()
             for chunk, off in raw_chunks:
                 view = memoryview(chunk).cast("B")
                 self.shared_memory.buf[off:off + view.nbytes] = view
 
-        # With a deferred announcement (pre_drain) nothing may touch the segment before
-        # it is out: immutable byte chunks are then written right after it, wherever it
-        # runs.  Host TENSORS are copied now (the caller announces first in that case:
-        # the training thread may change them as soon as this call returns).
-        raw_deferred = pre_drain is not None and bool(raw_chunks) and not host_ranges
-        if raw_deferred:
-            announce_only = pre_drain
-
-            def pre_drain():  # noqa: F811
-                announce_only()
-                write_raw()
-        else:
-            write_raw()
+        # The announcement (a pickle, and two socket round trips without a control
+        # segment) may wait for the completion thread only when nothing touches the
+        # segment before the drain: no host tensors (they are copied now, as the training
+        # thread may change them once this call returns), and the immutable byte chunks
+        # are written right after it.  The first announcement of a handler goes out
+        # inline: until it is out the agent's dict holds no step at all, and a SAVE event
+        # that overtakes it would find "no shard has a step"
+        # (ckpt_saver._check_shard_step_consistence).
+        may_hold = (announce is not None and not blocking and bool(device_ranges)
+                    and not host_ranges and self._announced_once)
+        held = announce_then_raw if may_hold else None
+        if held is None:
+            announce_then_raw()
+        if announce is not None:
+            self._announced_once = True
         if host_ranges:
             keep, ptrs, offs, lens = [], [], [], []
             for t, off, nbytes in host_ranges:
@@ -1140,11 +1104,10 @@ class SharedMemoryHandler:
         stager = None
         prepared = None
         if device_ranges:
-            stager = self._stager_for_ranges(device_ranges)
+            stager = self._stager_for([r[0] for r in device_ranges])
             # a dense repack of an oddly strided leaf runs on the CURRENT stream: do it
             # before a side stream is made to wait for that stream
-            prepared = prepared_hint if prepared_hint is not None else \
-                stager.prepare_ranges(device_ranges, keepalive)
+            prepared = stager.prepare_ranges(device_ranges, keepalive)
             if window is not None:
                 prepared = _clip_ranges(prepared, window[0], window[1])
                 if not prepared[0]:
@@ -1180,10 +1143,10 @@ class SharedMemoryHandler:
             if windowed and not stager.pinned():
                 stager.ctx.host_register(*stager._attached, prefault_threads=_host_threads())
                 stager._pin_started = True
-            hold = pre_drain is not None and not blocking and not windowed
-            if pre_drain is not None and not hold:
-                pre_drain()
-                pre_drain = None
+            if held is not None and (blocking or windowed):
+                held()
+                held = None
+            hold = held is not None
             if in_place and cut is not None:
                 ticket = plan.save_hybrid_async(host_addr, cut, stream, hold=hold)
             elif in_place:
@@ -1200,9 +1163,9 @@ class SharedMemoryHandler:
                 ev.record(stream)
                 self.last_pack_event = ev
             ctx = stager.ctx
-        if ctx is None and pre_drain is not None:
-            pre_drain()
-            pre_drain = None
+        if ctx is None and held is not None:  # the window held no device bytes
+            held()
+            held = None
         user_finish = finish or (lambda: None)
         if ctx is not None:
             def finish_and_pin():
@@ -1212,8 +1175,7 @@ class SharedMemoryHandler:
                 stager.pin_in_background()
         else:
             finish_and_pin = user_finish
-        pending = PendingSave(ctx, ticket, finish_and_pin, keepalive,
-                              pre_drain=pre_drain if ctx is not None else None,
+        pending = PendingSave(ctx, ticket, finish_and_pin, keepalive, announce=held,
                               on_error=on_error)
         self._pending = pending
         if blocking or ctx is None:
@@ -1339,36 +1301,17 @@ class SharedMemoryHandler:
             self.ensure_segment(lay.total)
         meta_dict = lay.meta
         conf: CheckpointConfig = meta_dict[DLROVER_CKPT_CONFIG_KEY]
-        conf.writing_shm = True
         unchanged = lay.unchanged and self._meta_published
         self._meta_published = False
-        self.metadata.payload_bytes = lay.total
 
         def announce():
             report_local_event(EventReportConstants.TYPE_INFO, str(conf.rank),
                                EventReportConstants.ACTION_MEM_CKPT_START, f"step={conf.step}")
-            self.metadata.next_unchanged = unchanged
-            self.metadata.set(meta_dict)
-
-        # Host-resident leaves are written by this thread right now, so the agent
-        # must already know the segment is changing.  With device leaves only,
-        # nothing touches the segment before the drain: the announcement (a
-        # pickle + two socket round trips) moves to the completion thread and
-        # the drain is held until it is out.
-        # The very first announcement of a handler is made inline: until it is out the
-        # agent's dict holds no step at all, and a SAVE event that overtakes it would
-        # find "no shard has a step" (ckpt_saver._check_shard_step_consistence).
-        defer_announce = ((not blocking) and bool(lay.device_leaves) and not lay.host_leaves
-                          and self._announced_once)
-        if not defer_announce:
-            announce()
-        self._announced_once = True
+            self._set_meta(meta_dict, True, unchanged, lay.total)
 
         def finish():
-            conf.writing_shm = False
-            self.metadata.next_unchanged = True  # the tree went out with the announcement
-            self.metadata.set(meta_dict)
-            self._meta_published = True
+            # the tree went out with the announcement
+            self._set_meta(meta_dict, False, True, lay.total)
             report_local_event(EventReportConstants.TYPE_INFO, str(conf.rank),
                                EventReportConstants.ACTION_MEM_CKPT_COMPLETE,
                                f"step={conf.step}")
@@ -1379,9 +1322,19 @@ class SharedMemoryHandler:
         keepalive = [state_dict] if lay.device_leaves else []
         return self.write_ranges(_triples(lay.device_leaves), _triples(lay.host_leaves),
                                  blocking=blocking, stream=stream, finish=finish,
-                                 keepalive=keepalive,
-                                 pre_drain=announce if defer_announce else None,
-                                 on_error=on_error)
+                                 keepalive=keepalive, announce=announce, on_error=on_error)
+
+    def _set_meta(self, meta_dict, writing: bool, unchanged: bool, payload_bytes: int):
+        """Publish the meta tree of the save in progress with writing_shm=`writing`:
+        True before the first byte of the segment changes, False once every byte has
+        landed.  unchanged: the meta plane already holds this tree (everything but the
+        CheckpointConfig), so only the header is rewritten."""
+        meta_dict[DLROVER_CKPT_CONFIG_KEY].writing_shm = writing
+        self.metadata.payload_bytes = payload_bytes
+        self.metadata.next_unchanged = unchanged
+        self._meta_published = False
+        self.metadata.set(meta_dict)
+        self._meta_published = not writing
 
     def save_shards_as_full(self, state_dict, coop: CoopContext, blocking: bool = True,
                             stream=None, on_complete=None, on_error=None):
@@ -1405,14 +1358,11 @@ class SharedMemoryHandler:
             try:
                 if total > 0:
                     self.ensure_segment(total)
-                conf.writing_shm = True
-                self.metadata.payload_bytes = total
-                self.metadata.next_unchanged = lay.unchanged and self._meta_published
-                self._meta_published = False
                 report_local_event(EventReportConstants.TYPE_INFO, str(conf.rank),
                                    EventReportConstants.ACTION_MEM_CKPT_START,
                                    f"step={conf.step}")
-                self.metadata.set(meta_dict)  # before any rank touches the segment
+                # before any rank touches the segment
+                self._set_meta(meta_dict, True, lay.unchanged and self._meta_published, total)
                 self._announced_once = True
             except BaseException:
                 coop.ctl.next_coop_seq(aborted=True)  # do not leave the others waiting
@@ -1431,10 +1381,7 @@ class SharedMemoryHandler:
                 if not coop.ctl.wait_slots(coop.n, coop.seq, coop.timeout):
                     raise RuntimeError("cooperative save: a local rank failed or did not "
                                        f"report its slice within {coop.timeout:.0f}s")
-                conf.writing_shm = False
-                self.metadata.next_unchanged = True
-                self.metadata.set(meta_dict)
-                self._meta_published = True
+                self._set_meta(meta_dict, False, True, total)
                 report_local_event(EventReportConstants.TYPE_INFO, str(conf.rank),
                                    EventReportConstants.ACTION_MEM_CKPT_COMPLETE,
                                    f"step={conf.step}")
@@ -1469,10 +1416,6 @@ class SharedMemoryHandler:
             if self._pending is None:  # raised before a completion thread took over
                 coop.ctl.slot_set(coop.index, coop.seq, ok=False)
             raise
-
-    def _run_completion(self, pending: PendingSave):
-        pending._complete()
-        self.last_timings = pending.timings
 
     # -- load ---------------------------------------------------------------------------
     def load_state_dict(self):

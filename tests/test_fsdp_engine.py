@@ -161,6 +161,30 @@ def test_engine_roundtrip_cuda(cuda_device, gloo, tmp_path, async_drain):
     _engine_roundtrip(tmp_path, "cuda", async_drain=async_drain)
 
 
+def test_failed_publication_gives_the_lock_back(gloo, tmp_path, monkeypatch):
+    """If the final writing_shm=False publication fails, the shard lock must not stay
+    ours (later saves would be skipped forever) and the error surfaces."""
+    engine = fe.FsdpCheckpointEngine(str(tmp_path), PosixDiskStorage(), async_drain=False)
+    paths = {"model_states": str(tmp_path / "1")}
+    calls = {"n": 0}
+    real_set = engine._shm_handler.metadata.set
+
+    def flaky_set(meta):
+        calls["n"] += 1
+        if calls["n"] == 2:  # the final writing_shm=False publication
+            raise RuntimeError("agent went away")
+        return real_set(meta)
+
+    monkeypatch.setattr(engine._shm_handler.metadata, "set", flaky_set)
+    with pytest.raises(RuntimeError):
+        engine.save_to_memory(1, _state(), paths)
+    saver = AsyncCheckpointSaver.get_ckpt_saver()
+    assert not saver._shm_locks[0].locked()
+    monkeypatch.setattr(engine._shm_handler.metadata, "set", real_set)
+    assert engine.save_to_memory(2, _state(), paths) is True
+    engine.close()
+
+
 def test_load_without_memory_or_files_returns_none(gloo, tmp_path):
     engine = fe.FsdpCheckpointEngine(str(tmp_path), PosixDiskStorage())
     assert engine.load() is None
