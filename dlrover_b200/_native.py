@@ -92,6 +92,10 @@ _SIGNATURES = {
     "fc_save_direct_async": (ctypes.c_int, [_vp, _vp, _vp, ctypes.c_int, ctypes.POINTER(_u64)]),
     "fc_save_hybrid_async": (ctypes.c_int, [_vp, _vp, _vp, _u64, ctypes.c_int,
                                             ctypes.POINTER(_u64)]),
+    "fc_save_delta_async": (ctypes.c_int, [_vp, _vp, _vp, ctypes.c_int, ctypes.POINTER(_u64)]),
+    "fc_save_delta_stats": (ctypes.c_int, [_vp, _u64, ctypes.POINTER(_u64),
+                                           ctypes.POINTER(ctypes.c_int)]),
+    "fc_delta_invalidate": (ctypes.c_int, [_vp]),
     "fc_save_sources_wait": (ctypes.c_int, [_vp, _u64]),
     "fc_restore_direct_async": (ctypes.c_int, [_vp, _vp, _vp]),
     "fc_plan_spans": (ctypes.c_int, [_vp, ctypes.POINTER(_u32)]),
@@ -272,6 +276,17 @@ class Plan:
                                                    _stream_ptr(compute_stream), int(cut),
                                                    int(hold), ctypes.byref(ticket)),
                "fc_save_hybrid_async")
+        return ticket.value
+
+    def save_delta_async(self, host_ptr: int, compute_stream=None, hold: bool = False) -> int:
+        """Incremental save: compare with the arena image of the last delta save of this
+        plan to `host_ptr` and drain only the work items that changed (a full save when
+        there is no such baseline).  See Context.save_delta_stats."""
+        ticket = _u64()
+        _check(load_library().fc_save_delta_async(self.handle, host_ptr,
+                                                  _stream_ptr(compute_stream), int(hold),
+                                                  ctypes.byref(ticket)),
+               "fc_save_delta_async")
         return ticket.value
 
     def restore_async(self, host_ptr: int, stream=None, direct: bool = False):
@@ -459,15 +474,32 @@ class Context:
         )
         return a.value, b.value, c.value
 
+    def save_delta_stats(self, ticket: int) -> Tuple[bool, int]:
+        """(incremental, drained bytes) of a drained save."""
+        nbytes, delta = _u64(), ctypes.c_int()
+        rc = _check(load_library().fc_save_delta_stats(self.handle, ticket, ctypes.byref(nbytes),
+                                                       ctypes.byref(delta)),
+                    "fc_save_delta_stats")
+        if rc == FC_ENOTREADY:
+            raise NativeError(rc, "fc_save_delta_stats", "the save has not drained yet")
+        return bool(delta.value), nbytes.value
+
+    def delta_invalidate(self):
+        """The next incremental save is a full one (something else wrote the arena or
+        the segment)."""
+        _check(load_library().fc_delta_invalidate(self.handle), "fc_delta_invalidate")
+
     def arena_fill(self, host_ptr: int, lo: int, hi: int, stream=None):
         """Host bytes [lo, hi) -> arena bytes [lo, hi); `stream` waits for them."""
         _check(load_library().fc_arena_fill(self.handle, host_ptr, int(lo), int(hi),
                                             _stream_ptr(stream)), "fc_arena_fill")
 
     def arena_tensor(self, nbytes: int):
-        """The first nbytes of the arena as a uint8 torch tensor (no copy)."""
+        """The first nbytes of the arena as a uint8 torch tensor (no copy).  Whoever
+        holds it may write the arena, so the incremental baseline is forgotten."""
         import torch
 
+        self.delta_invalidate()
         ptr, size = self.arena_info()
         if nbytes > size:
             raise NativeError(FC_EINVAL, "arena_tensor", "arena smaller than requested")

@@ -6,6 +6,14 @@
 //   fc_copy_tma_shift  TMA in, funnel shift shared->shared, TMA out: ranges whose
 //                      source and destination are not congruent mod 16
 // Pure byte copies; bound: HBM bandwidth, 2 bytes of traffic per checkpoint byte.
+// And the two gather-compare kernels of the incremental save (end of the file):
+//   fc_delta_tma       16-B congruent bodies: TMA loads of the source tile AND of the
+//                      arena tile it replaces, compare in shared memory, TMA store
+//                      only of the tiles that differ
+//   fc_delta_lsu       everything else (heads, tails, shifted ranges, small pieces):
+//                      copy_range with a compare, stores only the vectors that differ
+// Both write `seq` into dirty[item.pad0] when any byte of the item differs.
+// Traffic: 2 bytes read per checkpoint byte + 1 byte written per dirty byte.
 // Included by flashckpt.cu only.
 #pragma once
 
@@ -213,6 +221,7 @@ __device__ __forceinline__ void bulk_wait_all() {
 struct TileCursor {
   const FcItem* items;
   uint32_t n_items, item, off, n;
+  uint32_t idx;  // FcItem.pad0: index of the item's `all` entry (gather-compare only)
   uint64_t tptr, aoff;
   __device__ __forceinline__ void fetch() {
     if (item < n_items) {
@@ -221,6 +230,7 @@ struct TileCursor {
       tptr = ((uint64_t)a.y << 32) | a.x;
       aoff = ((uint64_t)a.w << 32) | a.z;
       n = b.x;
+      idx = b.y;
     }
   }
   __device__ __forceinline__ void init(const FcItem* it, uint32_t cnt) {
@@ -441,6 +451,219 @@ fc_copy_tma_shift(const FcItem* __restrict__ items, uint32_t n_items,
     }
     advance(cs);
     __syncthreads();
+  }
+  if (threadIdx.x == 0) bulk_wait_all();
+}
+
+// ---- gather-compare kernels (incremental save) -----------------------------------
+// The arena still holds the image the previous save drained to the segment.  These
+// kernels write into it only the bytes that differ from the new source bytes and mark
+// every `all` item that had any difference: dirty[item.pad0] = seq.  The host then
+// drains only the marked items.  A mark is the save's sequence number, so the marks
+// need no clearing between saves.
+
+// Plain (coherent) 128-bit load of arena bytes that this kernel may store to later.
+__device__ __forceinline__ uint4 ld_arena(const uint4* p) {
+  uint4 v;
+  asm volatile("ld.global.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+               : "l"(p));
+  return v;
+}
+
+__device__ __forceinline__ bool differ(const uint4& a, const uint4& b) {
+  return ((a.x ^ b.x) | (a.y ^ b.y) | (a.z ^ b.z) | (a.w ^ b.w)) != 0u;
+}
+
+// copy_shifted with a compare: the old vector is loaded with the source words and the
+// shifted result is stored only where it differs.  Returns this thread's "differs".
+template <int Q>
+__device__ __forceinline__ bool delta_shifted(const uint4* __restrict__ abase,
+                                              uint4* __restrict__ dst, uint32_t nvec,
+                                              uint32_t sh) {
+  constexpr int T = kLsuThreads, U = kLsuUnroll;
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t wbase = threadIdx.x - lane;
+  bool d = false;
+  for (uint32_t base = wbase; base < nvec; base += U * T) {  // warp-uniform bounds
+    uint4 lo[U], hi[U], old[U];
+#pragma unroll
+    for (int j = 0; j < U; ++j) {
+      const uint32_t idx = base + j * T + lane;
+      lo[j] = idx <= nvec ? ldg_stream(abase + idx) : make_uint4(0, 0, 0, 0);
+      hi[j] = (lane == 31u && idx < nvec) ? ldg_cached(abase + idx + 1) : make_uint4(0, 0, 0, 0);
+      old[j] = idx < nvec ? ld_arena(dst + idx) : make_uint4(0, 0, 0, 0);
+    }
+#pragma unroll
+    for (int j = 0; j < U; ++j) {
+      const uint4 nb = shfl_down1(lo[j]);
+      if (lane != 31u) hi[j] = nb;
+    }
+#pragma unroll
+    for (int j = 0; j < U; ++j) {
+      const uint32_t idx = base + j * T + lane;
+      if (idx < nvec) {
+        const uint4 v = funnel16<Q>(lo[j], hi[j], sh);
+        if (differ(v, old[j])) {
+          stg_stream(dst + idx, v);
+          d = true;
+        }
+      }
+    }
+  }
+  return d;
+}
+
+// copy_range with a compare (any alignment on either side).  Every thread of the CTA
+// must call it; returns this thread's "differs".
+__device__ __forceinline__ bool delta_range(const uint8_t* __restrict__ src,
+                                            uint8_t* __restrict__ dst, uint32_t n) {
+  constexpr int T = kLsuThreads, U = kLsuUnroll;
+  bool d = false;
+  uint32_t head = (uint32_t)((16u - ((uintptr_t)dst & 15u)) & 15u);
+  if (head > n) head = n;
+  if (threadIdx.x < head) {
+    const uint8_t v = src[threadIdx.x];
+    if (dst[threadIdx.x] != v) {
+      dst[threadIdx.x] = v;
+      d = true;
+    }
+  }
+  src += head;
+  dst += head;
+  n -= head;
+  const uint32_t nvec = n >> 4;
+  const uint32_t tail = n & 15u;
+  if (threadIdx.x < tail) {
+    const uint32_t o = (nvec << 4) + threadIdx.x;
+    const uint8_t v = src[o];
+    if (dst[o] != v) {
+      dst[o] = v;
+      d = true;
+    }
+  }
+  if (nvec == 0) return d;
+  const uint32_t r = (uint32_t)((uintptr_t)src & 15u);
+  uint4* __restrict__ dv = reinterpret_cast<uint4*>(dst);
+  if (r == 0) {
+    const uint4* __restrict__ s = reinterpret_cast<const uint4*>(src);
+    uint32_t i = threadIdx.x;
+    for (; i + (U - 1) * T < nvec; i += U * T) {
+      uint4 v[U], o[U];
+#pragma unroll
+      for (int j = 0; j < U; ++j) {
+        v[j] = ldg_stream(s + i + j * T);
+        o[j] = ld_arena(dv + i + j * T);
+      }
+#pragma unroll
+      for (int j = 0; j < U; ++j)
+        if (differ(v[j], o[j])) {
+          stg_stream(dv + i + j * T, v[j]);
+          d = true;
+        }
+    }
+    for (; i < nvec; i += T) {
+      const uint4 v = ldg_stream(s + i);
+      if (differ(v, ld_arena(dv + i))) {
+        stg_stream(dv + i, v);
+        d = true;
+      }
+    }
+    return d;
+  }
+  const uint4* __restrict__ ab = reinterpret_cast<const uint4*>(src - r);
+  const uint32_t sh = (r & 3u) * 8u;
+  switch (r >> 2) {
+    case 0: return delta_shifted<0>(ab, dv, nvec, sh) || d;
+    case 1: return delta_shifted<1>(ab, dv, nvec, sh) || d;
+    case 2: return delta_shifted<2>(ab, dv, nvec, sh) || d;
+    default: return delta_shifted<3>(ab, dv, nvec, sh) || d;
+  }
+}
+
+// Gather-compare for any item (residues, shifted ranges, pieces under 4 KiB; every item
+// under FC_VARIANT_LSU).  One CTA per item; a warp that saw a difference marks it.
+__global__ void __launch_bounds__(kLsuThreads)
+fc_delta_lsu(const FcItem* __restrict__ items, uint32_t n_items, uint8_t* __restrict__ arena,
+             uint32_t* __restrict__ dirty, uint32_t seq) {
+  for (uint32_t c = blockIdx.x; c < n_items; c += gridDim.x) {
+    const uint4 a = __ldg(reinterpret_cast<const uint4*>(items + c));
+    const uint4 b = __ldg(reinterpret_cast<const uint4*>(items + c) + 1);
+    const uint8_t* t = reinterpret_cast<const uint8_t*>(((uint64_t)a.y << 32) | a.x);
+    uint8_t* ar = arena + (((uint64_t)a.w << 32) | a.z);
+    const bool d = delta_range(t, ar, b.x);
+    if (__any_sync(0xffffffffu, d) && (threadIdx.x & 31u) == 0u) dirty[b.y] = seq;
+  }
+}
+
+// Gather-compare for the 16-B congruent bodies.  A stage holds the source tile and the
+// arena tile it replaces, both TMA-loaded on one mbarrier; the CTA compares them with
+// 128-bit shared-memory loads, and thread 0 TMA-stores the source tile only if it
+// differs.  Shared memory: stages x 2 x tile + one mbarrier per stage.
+constexpr int kDeltaThreads = 256;
+static inline size_t delta_smem_bytes(uint32_t tile, uint32_t stages) {
+  return (size_t)stages * 2u * tile + 8u * stages;
+}
+
+__global__ void __launch_bounds__(kDeltaThreads)
+fc_delta_tma(const FcItem* __restrict__ items, uint32_t n_items, uint8_t* __restrict__ arena,
+             uint32_t* __restrict__ dirty, uint32_t seq, uint32_t tile, uint32_t stages) {
+  extern __shared__ __align__(128) uint8_t fc_smem[];
+  const uint32_t smem_base = smem_u32(fc_smem);
+  const uint32_t bar_base = smem_base + stages * 2u * tile;
+  if (threadIdx.x == 0) {
+    for (uint32_t s = 0; s < stages; ++s) mbar_init(bar_base + 8 * s, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  __syncthreads();
+
+  // the load cursor is used by thread 0 only; the consume cursor is replicated
+  TileCursor ld, st;
+  ld.init(items, n_items);
+  st.init(items, n_items);
+
+  auto issue_load = [&](uint32_t stage) {  // thread 0
+    const uint32_t nb = ld.bytes(tile);
+    const uint32_t bar = bar_base + 8 * stage;
+    const uint32_t s_new = smem_base + stage * 2u * tile;
+    mbar_expect_tx(bar, 2u * nb);
+    bulk_g2s(s_new, reinterpret_cast<const void*>(ld.tptr + ld.off), nb, bar);
+    bulk_g2s(s_new + tile, arena + ld.aoff + ld.off, nb, bar);
+    ld.advance(tile);
+  };
+
+  if (threadIdx.x == 0) {
+    for (uint32_t s = 0; s < stages && ld.valid(); ++s) issue_load(s);
+  }
+
+  for (uint32_t k = 0; st.valid(); ++k) {
+    const uint32_t stage = k % stages;
+    mbar_wait(bar_base + 8 * stage, (k / stages) & 1u);
+    const uint32_t nb = st.bytes(tile);
+    const uint4* nw = reinterpret_cast<const uint4*>(fc_smem + (size_t)stage * 2u * tile);
+    const uint4* od = nw + tile / 16u;
+    bool d = false;
+    for (uint32_t i = threadIdx.x; i < nb / 16u; i += kDeltaThreads) d |= differ(nw[i], od[i]);
+    // every thread is done reading the stage (and the one before it) past this point
+    const bool tile_dirty = __syncthreads_or(d) != 0;
+    if (threadIdx.x == 0) {
+      if (tile_dirty) {
+        bulk_s2g(arena + st.aoff + st.off, smem_base + stage * 2u * tile, nb);
+        bulk_commit();
+        dirty[st.idx] = seq;
+      }
+      if (k >= 1 && ld.valid()) {
+        // refill the stage consumed at k-1 once its store (if any) has read it out;
+        // only committed stores count as groups
+        if (tile_dirty)
+          bulk_wait_read<1>();
+        else
+          bulk_wait_read<0>();
+        issue_load((k - 1) % stages);
+      }
+    }
+    st.advance(tile);
   }
   if (threadIdx.x == 0) bulk_wait_all();
 }

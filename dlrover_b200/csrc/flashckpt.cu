@@ -31,6 +31,9 @@
 //   fc_copy_lsu       256-thread CTAs, 128-bit LDG/STG, 4-way unrolled: heads,
 //                     tails, tiny ranges, the bounded-arena windows, and
 //                     everything when FC_VARIANT_LSU is selected.
+// and, for the opt-in incremental save (fc_save_delta_async), their gather-compare
+// twins fc_delta_tma / fc_delta_lsu: they write only the bytes that differ from the
+// arena's previous image and mark the work items to drain.
 //
 // No torch types here; see include/flashckpt.h for the ABI contract.
 
@@ -92,6 +95,24 @@ extern "C" const char* fc_last_error(void) { return g_err; }
 
 // ----------------------------------------------------------------- host side --
 
+// What the drain of an incremental save needs to turn dirty marks into DMA runs: the
+// extent of every `all` item (ascending arena offset) and the plan's runs (arena offset
+// -> segment offset).  Built once per plan fill and shared with the queued drain jobs,
+// so a plan update or destroy never pulls it from under a drain.
+struct DeltaMap {
+  std::vector<uint64_t> aoff;
+  std::vector<uint32_t> len;
+  std::vector<FcRun> runs;
+  bool same_extents(const DeltaMap& o) const {
+    if (aoff != o.aoff || len != o.len || runs.size() != o.runs.size()) return false;
+    for (size_t i = 0; i < runs.size(); ++i)
+      if (runs[i].off != o.runs[i].off || runs[i].len != o.runs[i].len ||
+          runs[i].hoff != o.runs[i].hoff)
+        return false;
+    return true;
+  }
+};
+
 struct fc_ctx {
   int device = 0;
   int sm_count = 132;
@@ -152,6 +173,9 @@ struct fc_ctx {
     bool direct = false;
     uint64_t arena_base = 0;  // arena byte 0 holds this segment offset (hybrid: the cut)
     uint64_t ticket = 0;
+    // incremental save: `runs` is built by the pump from the items marked `seq`
+    std::shared_ptr<const DeltaMap> delta;
+    uint32_t seq = 0;
   };
   uint64_t direct_ticket = 0;  // last ticket with an in-place part (sources frozen until drained)
   uint64_t inplace_done_ticket = 0;  // last ticket whose in-place part has left the tensors
@@ -169,7 +193,33 @@ struct fc_ctx {
   std::vector<void*> dead_dev, dead_pinned;
   uint64_t drain_piece = kDrainPiece;
   int drain_depth = kDrainDepth;
+  // Incremental saves (fc_save_delta_async).  The baseline is the (plan, host_base) of
+  // the last delta save that drained without error: the arena then is a byte image of
+  // what the segment holds for that plan.  Every other operation that writes the arena
+  // or the segment through this context forgets it (delta_forget).  Guarded by `mu`.
+  const fc_plan* base_plan = nullptr;
+  const uint8_t* base_host = nullptr;
+  bool base_valid = false;
+  uint64_t base_ticket = 0;  // the delta save that becomes the baseline once drained
+  // dirty marks: one entry per `all` item of the plan being saved, = the save's seq
+  uint32_t* dirty = nullptr;
+  uint32_t* dirty_pinned = nullptr;
+  uint32_t dirty_cap = 0;
+  uint32_t delta_seq = 0;
+  // what the drain of ticket stat_ticket moved
+  uint64_t stat_ticket = 0, stat_bytes = 0;
+  int stat_delta = 0;
 };
+
+static void delta_forget_locked(fc_ctx* c) {
+  c->base_valid = false;
+  c->base_ticket = 0;
+}
+
+static void delta_forget(fc_ctx* c) {
+  std::lock_guard<std::mutex> lk(c->mu);
+  delta_forget_locked(c);
+}
 
 static fc_ctx::HostReg* reg_covering(fc_ctx* c, const uint8_t* p, uint64_t len);
 
@@ -297,6 +347,35 @@ static cudaError_t stage_run(fc_ctx* c, const std::vector<StagePiece>& pieces, b
   return (cudaError_t)err.load();
 }
 
+// Incremental save: fetch the dirty marks once the gather-compare kernels are done and
+// turn the items marked job.seq into runs, merged where both the arena and the segment
+// continue.  Item i lies inside one plan run, which maps its arena offset to the segment.
+static cudaError_t delta_runs(fc_ctx* c, fc_ctx::DrainJob& job) {
+  const DeltaMap& m = *job.delta;
+  const size_t n = m.aoff.size();
+  job.runs.clear();
+  if (n == 0) return cudaSuccess;
+  cudaError_t e = cudaMemcpyAsync(c->dirty_pinned, c->dirty, n * sizeof(uint32_t),
+                                  cudaMemcpyDeviceToHost, c->copy_stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(c->copy_stream);
+  if (e != cudaSuccess) return e;
+  size_t r = 0;
+  for (size_t i = 0; i < n; ++i) {
+    if (c->dirty_pinned[i] != job.seq) continue;
+    while (m.runs[r].off + m.runs[r].len <= m.aoff[i]) ++r;
+    const uint64_t hoff = m.runs[r].hoff + (m.aoff[i] - m.runs[r].off);
+    if (!job.runs.empty()) {
+      FcRun& last = job.runs.back();
+      if (last.off + last.len == m.aoff[i] && last.hoff + last.len == hoff) {
+        last.len += m.len[i];
+        continue;
+      }
+    }
+    job.runs.push_back({m.aoff[i], m.len[i], hoff});
+  }
+  return cudaSuccess;
+}
+
 static void pump_main(fc_ctx* c) {
   cudaSetDevice(c->device);
   for (;;) {
@@ -313,6 +392,11 @@ static void pump_main(fc_ctx* c) {
     }
     cudaError_t e = cudaStreamWaitEvent(c->copy_stream, c->ev_pack_end, 0);
     if (e == cudaSuccess) e = cudaEventRecord(c->ev_drain_start, c->copy_stream);
+    if (job.delta && e == cudaSuccess) e = delta_runs(c, job);
+    uint64_t drained = 0;
+    for (const FcRun& r : job.runs) drained += r.len;
+    for (const FcSpan& sp : job.spans) drained += sp.len;
+    const bool delta = job.delta != nullptr;
     const int depth = std::max(1, std::min(c->drain_depth, kDrainRing));
     uint64_t k = 0, copies = 0;
     if (job.staged_threads > 0 && e == cudaSuccess) {
@@ -419,7 +503,13 @@ static void pump_main(fc_ctx* c) {
         c->drain_rc = FC_ECUDA;
         c->drain_err = std::string("drain pump: ") + cudaGetErrorString(e);
         (void)cudaGetLastError();
+        delta_forget_locked(c);
+      } else if (job.ticket == c->base_ticket) {
+        c->base_valid = true;  // the segment now holds the arena's image of this plan
       }
+      c->stat_ticket = job.ticket;
+      c->stat_bytes = drained;
+      c->stat_delta = delta ? 1 : 0;
       c->drained_ticket = job.ticket;
     }
     c->cv.notify_all();
@@ -456,6 +546,7 @@ struct fc_plan {
   // and windowed saves launch the TMA kernels over such slices.
   std::vector<uint32_t> pos_bulk, pos_resid, pos_shift;
   std::vector<FcSpan> spans;  // source ranges by arena offset (in-place save / restore)
+  std::shared_ptr<const DeltaMap> dmap;  // item extents + runs for the incremental drain
   cudaEvent_t ev_upload = nullptr;  // last table upload
   cudaEvent_t ev_last_use = nullptr;  // last kernel that read the tables
 };
@@ -569,6 +660,8 @@ extern "C" int fc_ctx_destroy(fc_ctx* c) {
   if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
   if (c->copy_stream2) cudaStreamDestroy(c->copy_stream2);
   if (c->arena) cudaFree(c->arena);
+  if (c->dirty) cudaFree(c->dirty);
+  if (c->dirty_pinned) cudaFreeHost(c->dirty_pinned);
   for (void* q : c->dead_dev) cudaFree(q);
   for (void* q : c->dead_pinned) cudaFreeHost(q);
   delete c;
@@ -599,6 +692,7 @@ extern "C" int fc_arena_reserve(fc_ctx* c, uint64_t bytes) {
   if (rc) return rc;
   if (c->save_inflight || c->restore_inflight)
     return fail(FC_EBUSY, "fc_arena_reserve: arena in use%s%s");
+  delta_forget(c);  // the new arena holds no image of the segment
   if (c->arena) {
     FC_CUDA(cudaFree(c->arena));
     c->arena = nullptr;
@@ -1042,6 +1136,9 @@ static int plan_fill(fc_plan* p, uint32_t n, const void* const* dev_ptrs,
   if (all.size() > 0xFFFFFFF0ull) return fail(FC_EINVAL, "plan: too many work items%s%s");
   std::stable_sort(all.begin(), all.end(),
                    [](const FcItem& a, const FcItem& b) { return a.aoff < b.aoff; });
+  // every item, and every piece derived from it below, carries the index of its `all`
+  // entry: the gather-compare kernels mark dirty[pad0]; the copy kernels ignore it
+  for (size_t k = 0; k < all.size(); ++k) all[k].pad0 = (uint32_t)k;
   // Derive the TMA-variant tables from `all`, item by item.  Interior item
   // boundaries are 128-B aligned in arena space, so a head (< 16 B) only exists at
   // the start of a range and a tail only at its end.
@@ -1101,6 +1198,21 @@ static int plan_fill(fc_plan* p, uint32_t n, const void* const* dev_ptrs,
       if (by_host[i].off < by_host[i - 1].off + by_host[i - 1].len)
         return fail(FC_EINVAL, "plan: tensors overlap in the segment%s%s");
   }
+  std::shared_ptr<DeltaMap> dmap = std::make_shared<DeltaMap>();
+  dmap->aoff.reserve(all.size());
+  dmap->len.reserve(all.size());
+  for (const FcItem& it : all) {
+    dmap->aoff.push_back(it.aoff);
+    dmap->len.push_back(it.nbytes);
+  }
+  dmap->runs = runs;
+  // re-targeting the tensors (same extents) keeps an incremental baseline; anything
+  // that moves a byte of the image does not
+  if (!p->dmap || !p->dmap->same_extents(*dmap)) {
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (c->base_plan == p) delta_forget_locked(c);
+  }
+  p->dmap = std::move(dmap);
   p->runs.swap(runs);
   p->h_all.swap(all);
   p->pos_bulk.swap(pos_bulk);
@@ -1208,6 +1320,13 @@ extern "C" int fc_plan_destroy(fc_plan* p) {
   // the whole device) and defer the cudaFree (which would sync everything).
   if (p->ev_last_use) cudaEventSynchronize(p->ev_last_use);
   if (p->ev_upload) cudaEventSynchronize(p->ev_upload);
+  {
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (c->base_plan == p) {
+      delta_forget_locked(c);
+      c->base_plan = nullptr;  // a later plan may be allocated at the same address
+    }
+  }
   for (FcTable* t : {&p->all, &p->bulk, &p->resid, &p->shift}) {
     if (t->dev) c->dead_dev.push_back(t->dev);
     if (t->pinned) c->dead_pinned.push_back(t->pinned);
@@ -1351,12 +1470,14 @@ static int launch_copy(fc_plan* p, cudaStream_t s, int variant) {
 extern "C" int fc_pack_async(fc_plan* p, void* stream, int variant) {
   if (!p) return fail(FC_EINVAL, "fc_pack_async: null plan%s%s");
   FC_GUARD(p->ctx);
+  delta_forget(p->ctx);
   return launch_copy<0>(p, (cudaStream_t)stream, variant);
 }
 
 extern "C" int fc_unpack_async(fc_plan* p, void* stream, int variant) {
   if (!p) return fail(FC_EINVAL, "fc_unpack_async: null plan%s%s");
   FC_GUARD(p->ctx);
+  delta_forget(p->ctx);
   return launch_copy<1>(p, (cudaStream_t)stream, variant);
 }
 
@@ -1501,6 +1622,11 @@ extern "C" int fc_save_cancel(fc_ctx* c, uint64_t ticket) {
         c->jobs.erase(it);
         break;
       }
+    // the gather has changed the arena, the segment keeps the previous image
+    delta_forget_locked(c);
+    c->stat_ticket = ticket;
+    c->stat_bytes = 0;
+    c->stat_delta = 0;
     c->held_ticket = 0;
     c->drained_ticket = std::max(c->drained_ticket, ticket);  // nothing will be written
     if (c->direct_ticket == ticket) c->inplace_done_ticket = ticket;
@@ -1518,6 +1644,7 @@ static int save_async_impl(fc_plan* p, void* host_base, void* compute_stream, ui
   if (rc) return rc;
   if (c->save_inflight || c->restore_inflight)
     return fail(FC_EBUSY, "fc_save_async: previous save/restore still draining%s%s");
+  delta_forget(c);
   cudaStream_t cs = (cudaStream_t)compute_stream;
   if (p->arena_end > c->arena_bytes) {
     if (c->arena_bytes < (8ull << 20) || !p->identity)
@@ -1526,6 +1653,9 @@ static int save_async_impl(fc_plan* p, void* host_base, void* compute_stream, ui
     if (rc) return rc;
     std::lock_guard<std::mutex> lk(c->mu);
     c->ticket += 1;
+    c->stat_ticket = c->ticket;
+    c->stat_bytes = p->payload;
+    c->stat_delta = 0;
     c->drained_ticket = c->ticket;  // already complete
     if (ticket) *ticket = c->ticket;
     return FC_OK;
@@ -1577,6 +1707,7 @@ static int save_hybrid_impl(fc_plan* p, void* host_base, void* compute_stream, u
   if (rc) return rc;
   if (c->save_inflight || c->restore_inflight)
     return fail(FC_EBUSY, "fc_save_hybrid_async: previous save/restore still draining%s%s");
+  delta_forget(c);
   if (!p->identity && cut != ~0ull)
     return fail(FC_EINVAL, "fc_save_hybrid_async: needs a plan whose arena is an image of "
                            "the segment%s%s");
@@ -1647,6 +1778,157 @@ extern "C" int fc_save_direct_async(fc_plan* p, void* host_base, void* compute_s
   return save_hybrid_impl(p, host_base, compute_stream, ~0ull, hold, ticket);
 }
 
+// ---- incremental save --------------------------------------------------------------
+
+static int check_ticket(fc_ctx* c, uint64_t ticket, const char* who);
+
+static int launch_delta_lsu(fc_ctx* c, const FcItem* items, uint32_t n, cudaStream_t s,
+                            uint32_t seq) {
+  if (n == 0) return FC_OK;
+  uint32_t grid = std::min<uint32_t>(n, (uint32_t)(c->sm_count * c->lsu_ctas_per_sm));
+  fc_delta_lsu<<<grid, kLsuThreads, 0, s>>>(items, n, c->arena, c->dirty, seq);
+  FC_CUDA(cudaGetLastError());
+  c->n_kernels += 1;
+  return FC_OK;
+}
+
+// The ring takes the copy ring's shared memory (fc_set_launch): a stage holds a source
+// and an old tile of half the copy tile each (default 2 stages x 2 x 48 KiB).
+static int launch_delta_tma(fc_ctx* c, const FcItem* items, uint32_t n, cudaStream_t s,
+                            uint32_t seq) {
+  if (n == 0) return FC_OK;
+  const uint32_t tile = std::max<uint32_t>(128u, ((uint32_t)c->tma_tile / 2u) & ~127u);
+  const uint32_t stages = (uint32_t)c->tma_stages;
+  const size_t smem = delta_smem_bytes(tile, stages);
+  FC_CUDA(cudaFuncSetAttribute(fc_delta_tma, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)smem));
+  uint32_t grid = std::min<uint32_t>(n, (uint32_t)(c->sm_count * c->tma_ctas_per_sm));
+  fc_delta_tma<<<grid, kDeltaThreads, smem, s>>>(items, n, c->arena, c->dirty, seq, tile, stages);
+  FC_CUDA(cudaGetLastError());
+  c->n_kernels += 1;
+  return FC_OK;
+}
+
+// Gather-compare over the whole plan: bulk bodies through the TMA ring, shifted ranges
+// and residues through the LSU kernel (FC_VARIANT_LSU: every item through the LSU kernel).
+static int launch_delta(fc_plan* p, cudaStream_t s, uint32_t seq) {
+  fc_ctx* c = p->ctx;
+  FC_CUDA(cudaStreamWaitEvent(s, p->ev_upload, 0));
+  int rc;
+  if (c->variant == FC_VARIANT_TMA) {
+    rc = launch_delta_tma(c, p->bulk.dev, p->bulk.n, s, seq);
+    if (!rc) rc = launch_delta_lsu(c, p->shift.dev, p->shift.n, s, seq);
+    if (!rc) rc = launch_delta_lsu(c, p->resid.dev, p->resid.n, s, seq);
+  } else {
+    rc = launch_delta_lsu(c, p->all.dev, p->all.n, s, seq);
+  }
+  if (rc) return rc;
+  FC_CUDA(cudaEventRecord(p->ev_last_use, s));
+  return FC_OK;
+}
+
+extern "C" int fc_save_delta_async(fc_plan* p, void* host_base, void* compute_stream, int hold,
+                                   uint64_t* ticket) {
+  if (!p || (!host_base && p->payload))
+    return fail(FC_EINVAL, "fc_save_delta_async: null argument%s%s");
+  fc_ctx* c = p->ctx;
+  FC_GUARD(c);
+  int rc = refresh_inflight(c);
+  if (rc) return rc;
+  if (c->save_inflight || c->restore_inflight)
+    return fail(FC_EBUSY, "fc_save_delta_async: previous save/restore still draining%s%s");
+  if (p->arena_end > c->arena_bytes)
+    return fail(FC_EINVAL, "fc_save_delta_async: the arena must hold the whole plan (no "
+                           "incremental bounded-arena save)%s%s");
+  uint8_t* host = static_cast<uint8_t*>(host_base);
+  bool delta;
+  {
+    std::lock_guard<std::mutex> lk(c->mu);
+    // a sticky drain error must surface BEFORE the arena is overwritten
+    if (c->drain_rc != FC_OK) return fail(c->drain_rc, "%s", c->drain_err.c_str());
+    delta = c->base_valid && c->base_plan == p && c->base_host == host;
+    delta_forget_locked(c);  // the arena changes now; valid again once this save drained
+  }
+  cudaStream_t cs = (cudaStream_t)compute_stream;
+  const uint32_t n_all = p->all.n;
+  bool reset = false;
+  if (delta && n_all > c->dirty_cap) {
+    const uint32_t cap = (uint32_t)std::min<uint64_t>(0xFFFFFFF0ull, n_all + n_all / 4 + 16);
+    uint32_t* nd = nullptr;
+    uint32_t* np = nullptr;
+    cudaError_t e = cudaMalloc(&nd, (size_t)cap * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaHostAlloc(&np, (size_t)cap * sizeof(uint32_t), cudaHostAllocDefault);
+    if (e != cudaSuccess) {
+      (void)cudaGetLastError();
+      if (nd) c->dead_dev.push_back(nd);
+      return fail(FC_ENOMEM, "dirty marks alloc: %s", cudaGetErrorString(e));
+    }
+    if (c->dirty) c->dead_dev.push_back(c->dirty);  // no save is in flight: nothing reads them
+    if (c->dirty_pinned) c->dead_pinned.push_back(c->dirty_pinned);
+    c->dirty = nd;
+    c->dirty_pinned = np;
+    c->dirty_cap = cap;
+    reset = true;
+  }
+  if (delta) {
+    // marks are sequence numbers: cleared only for a fresh array or when seq wraps
+    if (++c->delta_seq == 0) reset = true;
+    if (reset) {
+      FC_CUDA(cudaMemsetAsync(c->dirty, 0, (size_t)c->dirty_cap * sizeof(uint32_t), cs));
+      c->delta_seq = 1;
+    }
+  }
+  FC_CUDA(cudaEventRecord(c->ev_pack_start, cs));
+  rc = delta ? launch_delta(p, cs, c->delta_seq) : launch_copy<0>(p, cs, FC_VARIANT_AUTO);
+  if (rc) return rc;
+  FC_CUDA(cudaEventRecord(c->ev_pack_end, cs));
+  const int staged =
+      p->runs.empty() ? 0 : staged_threads_for(c, host + p->host_lo, p->host_hi - p->host_lo);
+  {
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (c->drain_rc != FC_OK) return fail(c->drain_rc, "%s", c->drain_err.c_str());
+    if (!c->pump.joinable()) c->pump = std::thread(pump_main, c);
+    c->ticket += 1;
+    fc_ctx::DrainJob job;
+    job.staged_threads = staged;
+    job.host = host;
+    if (delta) {
+      job.delta = p->dmap;
+      job.seq = c->delta_seq;
+    } else {
+      job.runs = p->runs;
+    }
+    job.ticket = c->ticket;
+    if (hold) c->held_ticket = c->ticket;
+    c->jobs.push_back(std::move(job));
+    c->save_inflight = true;
+    c->base_plan = p;
+    c->base_host = host;
+    c->base_ticket = c->ticket;
+    if (ticket) *ticket = c->ticket;
+  }
+  c->cv.notify_all();
+  return FC_OK;
+}
+
+extern "C" int fc_save_delta_stats(fc_ctx* c, uint64_t ticket, uint64_t* drained_bytes,
+                                   int* delta) {
+  int rc = check_ticket(c, ticket, "fc_save_delta_stats");
+  if (rc) return rc;
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (c->drained_ticket < ticket) return FC_ENOTREADY;
+  if (c->stat_ticket != ticket) return fail(FC_EINVAL, "fc_save_delta_stats: no statistics%s%s");
+  if (drained_bytes) *drained_bytes = c->stat_bytes;
+  if (delta) *delta = c->stat_delta;
+  return FC_OK;
+}
+
+extern "C" int fc_delta_invalidate(fc_ctx* c) {
+  if (!c) return fail(FC_EINVAL, "fc_delta_invalidate: null ctx%s%s");
+  delta_forget(c);
+  return FC_OK;
+}
+
 extern "C" int fc_restore_direct_async(fc_plan* p, const void* host_base, void* stream) {
   if (!p || (!host_base && p->payload))
     return fail(FC_EINVAL, "fc_restore_direct_async: null argument%s%s");
@@ -1656,6 +1938,7 @@ extern "C" int fc_restore_direct_async(fc_plan* p, const void* host_base, void* 
   if (rc) return rc;
   if (c->save_inflight || c->restore_inflight)
     return fail(FC_EBUSY, "fc_restore_direct_async: context busy%s%s");
+  delta_forget(c);
   cudaStream_t s = (cudaStream_t)stream;
   const uint8_t* hb = static_cast<const uint8_t*>(host_base);
   // the targets may still be read by work queued on `stream`
@@ -1925,6 +2208,7 @@ extern "C" int fc_restore_async(fc_plan* p, const void* host_base, void* stream)
   if (rc) return rc;
   if (c->save_inflight || c->restore_inflight)
     return fail(FC_EBUSY, "fc_restore_async: arena busy%s%s");
+  delta_forget(c);
   if (p->arena_end > c->arena_bytes) {
     if (c->arena_bytes < (8ull << 20) || !p->identity)
       return fail(FC_EINVAL, "arena smaller than the plan: call fc_arena_reserve first%s%s");
@@ -1978,6 +2262,7 @@ extern "C" int fc_arena_fill(fc_ctx* c, const void* host_base, uint64_t lo, uint
   if (rc) return rc;
   if (c->save_inflight || c->restore_inflight)
     return fail(FC_EBUSY, "fc_arena_fill: arena busy%s%s");
+  delta_forget(c);
   if (hi > c->arena_bytes) return fail(FC_EINVAL, "fc_arena_fill: arena too small%s%s");
   if (hi == lo) return FC_OK;
   cudaStream_t s = (cudaStream_t)stream;

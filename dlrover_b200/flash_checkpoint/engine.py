@@ -644,6 +644,18 @@ class CheckpointEngine(metaclass=ABCMeta):
     def in_place_snapshot_bytes(self, value: int):
         self._shm_handler.in_place_snapshot_bytes = int(value)
 
+    # Incremental saves (opt-in; also DLROVER_B200_INCREMENTAL=1): a full-snapshot save
+    # compares the state with the image the previous save left in the HBM arena and
+    # drains only the chunks that changed (a frozen base model does not cross PCIe
+    # again).  The segment's bytes are the same as without it.
+    @property
+    def incremental(self) -> bool:
+        return self._shm_handler.incremental
+
+    @incremental.setter
+    def incremental(self, value: bool):
+        self._shm_handler.incremental = bool(value)
+
     def wait_snapshot(self):
         """Call before the first write to tensors handed to the last save."""
         self._shm_handler.wait_snapshot()
@@ -736,6 +748,11 @@ class CheckpointEngine(metaclass=ABCMeta):
     def last_save_timings(self):
         """(pack_ms, drain_ms, total_ms) device times of the last finished save."""
         return self._shm_handler.last_timings
+
+    def last_save_stats(self):
+        """{"delta": bool, "drained_bytes": int} of the last finished save when it went
+        through the incremental path (delta False: it was a full save), else None."""
+        return self._shm_handler.last_save_stats
 
     # -- memory load ---------------------------------------------------------------------
     def get_state_dict_from_memory(self):

@@ -676,10 +676,11 @@ class PendingSave:
 
     def __init__(self, ctx: Optional[native.Context], ticket: int, finish: Callable[[], None],
                  keepalive: list, announce: Optional[Callable[[], None]] = None,
-                 on_error: Optional[Callable[[], None]] = None):
+                 on_error: Optional[Callable[[], None]] = None, delta: bool = False):
         self._on_error = on_error
         self._ctx = ctx
         self._ticket = ticket
+        self._delta = delta  # issued through save_delta_async: `stats` is filled in
         self._finish = finish
         self._keepalive = keepalive
         self._announce = announce  # set <=> the drain is held until it has run
@@ -687,6 +688,7 @@ class PendingSave:
         self._error: Optional[BaseException] = None
         self._lock = threading.Lock()
         self.timings: Optional[Tuple[float, float, float]] = None
+        self.stats: Optional[Dict[str, Any]] = None
 
     def _complete(self):
         """Wait for the DMA, then close the protocol.  Runs exactly once."""
@@ -708,6 +710,9 @@ class PendingSave:
                 if self._ctx is not None:
                     self._ctx.save_wait(self._ticket)
                     self.timings = self._ctx.save_timings(self._ticket)
+                    if self._delta:
+                        was_delta, nbytes = self._ctx.save_delta_stats(self._ticket)
+                        self.stats = {"delta": was_delta, "drained_bytes": nbytes}
                 self._finish()
             except BaseException as e:  # surfaced by wait()
                 self._error = e
@@ -897,6 +902,12 @@ class SharedMemoryHandler:
         # is drained in place first): shortens the time the tensors stay frozen
         self.in_place_snapshot_bytes = int(os.getenv("DLROVER_B200_IN_PLACE_SNAPSHOT_MB", "0")) << 20
         self.last_save_in_place = False
+        # incremental saves: opt-in, see write_ranges
+        self.incremental = os.getenv("DLROVER_B200_INCREMENTAL", "0") == "1"
+        # {"delta": bool, "drained_bytes": int} of the last finished save when it went
+        # through the incremental path (None for any other save)
+        self.last_save_stats: Optional[Dict[str, Any]] = None
+        self._delta_segment = None  # the mapping the last incremental save wrote to
         self.last_restore_stats: Dict[str, float] = {}
         self.last_hybrid_cut = None
         self._snapshot_ceiling = 0  # largest snapshot arena HBM turned out to have room for
@@ -954,7 +965,14 @@ class SharedMemoryHandler:
                 self._stager.detach()
             shm.close()
             self.shared_memory = None
+        self._delta_invalidate()
         self.init_shared_memory(create=False)
+
+    def _delta_invalidate(self):
+        """The segment was (re-)mapped: the next incremental save must be a full one."""
+        self._delta_segment = None
+        if self._stager is not None:
+            self._stager.ctx.delta_invalidate()
 
     def _create_tensor_meta(self, value):
         """Meta of one leaf at the current end of the layout (API parity with
@@ -1031,6 +1049,7 @@ class SharedMemoryHandler:
         if self.shared_memory is not None:
             self.shared_memory.close()
             self.shared_memory = None
+        self._delta_invalidate()
         self.init_shared_memory(create=True, size=total)
         self._buffer_size = total
 
@@ -1103,6 +1122,7 @@ class SharedMemoryHandler:
         ctx, ticket = None, 0
         stager = None
         prepared = None
+        delta = False
         if device_ranges:
             stager = self._stager_for([r[0] for r in device_ranges])
             # a dense repack of an oddly strided leaf runs on the CURRENT stream: do it
@@ -1147,10 +1167,20 @@ class SharedMemoryHandler:
                 held()
                 held = None
             hold = held is not None
+            # incremental saves need an arena image of the whole plan to compare with:
+            # full-snapshot saves only (not in place, not hybrid, not windowed)
+            delta = self.incremental and not in_place and arena == stager.ARENA_FULL
+            if delta and (self._delta_segment is not self.shared_memory
+                          or self.shared_memory.stale()):
+                # another mapping than the one the baseline was drained to
+                stager.ctx.delta_invalidate()
             if in_place and cut is not None:
                 ticket = plan.save_hybrid_async(host_addr, cut, stream, hold=hold)
             elif in_place:
                 ticket = plan.save_direct_async(host_addr, stream, hold=hold)
+            elif delta:
+                ticket = plan.save_delta_async(host_addr, stream, hold=hold)
+                self._delta_segment = self.shared_memory
             else:
                 ticket = plan.save_async(host_addr, stream, hold=hold)
             self._last_ticket = (stager.ctx, ticket)
@@ -1175,12 +1205,20 @@ class SharedMemoryHandler:
                 stager.pin_in_background()
         else:
             finish_and_pin = user_finish
+        if delta and ctx is not None:
+            pin_after = finish_and_pin
+
+            def finish_and_pin():
+                # visible before the caller's completion callback and before wait() returns
+                self.last_save_stats = pending.stats
+                pin_after()
         pending = PendingSave(ctx, ticket, finish_and_pin, keepalive, announce=held,
-                              on_error=on_error)
+                              on_error=on_error, delta=ctx is not None and delta)
         self._pending = pending
         if blocking or ctx is None:
             pending._complete()
             self.last_timings = pending.timings
+            self.last_save_stats = pending.stats
             self._pending = None
             pending.wait()  # re-raise a drain error
             return None
@@ -1206,6 +1244,7 @@ class SharedMemoryHandler:
                     pending._complete()
                     if handler is not None:
                         handler.last_timings = pending.timings
+                        handler.last_save_stats = pending.stats
                     del handler
 
             threading.Thread(target=loop, name="fc-drain", daemon=True).start()
@@ -1271,6 +1310,7 @@ class SharedMemoryHandler:
             if shm is not None:
                 shm.close()
                 self.shared_memory = None
+            self._delta_invalidate()
             self.init_shared_memory(create=False)
         if self.shared_memory is None or self.shared_memory.size != total:
             have = None if self.shared_memory is None else self.shared_memory.size

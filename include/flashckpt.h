@@ -228,6 +228,30 @@ int fc_save_direct_async(fc_plan* plan, void* host_base, void* compute_stream, i
  * (The reference keeps the sources frozen for the whole copy, ckpt_saver.py:198-231.) */
 int fc_save_hybrid_async(fc_plan* plan, void* host_base, void* compute_stream, uint64_t cut,
                          int hold, uint64_t* ticket);
+/* Incremental save (opt-in).  After a save has drained, the arena is a byte image of
+ * the segment; the next save of the same plan to the same host_base compares every new
+ * byte with the arena byte it replaces (gather-compare kernels: 2 bytes read per
+ * checkpoint byte + 1 written per changed byte), writes only what differs and drains
+ * only the work items (<= chunk_bytes each) that had a difference.  The segment ends up
+ * byte-identical to what fc_save_async writes.
+ * The comparison is against a BASELINE: the (plan, host_base) of the last delta save
+ * that drained without error.  Without a baseline the call is a normal full gather +
+ * drain, which then becomes the baseline.  The library forgets the baseline whenever
+ * the arena or the segment may no longer hold that image: arena reallocation, any
+ * other save / restore / pack / unpack / fc_arena_fill, fc_save_cancel, a drain error,
+ * fc_plan_destroy of the baseline plan, and an fc_plan_update* that changes the
+ * (arena offset, segment offset, length) of any range (re-targeting the tensor
+ * pointers alone keeps it).  A writer of the segment outside this context must call
+ * fc_delta_invalidate.  The arena must hold the whole plan (no bounded-arena mode:
+ * FC_EINVAL).  hold != 0: as fc_save_async_held. */
+int fc_save_delta_async(fc_plan* plan, void* host_base, void* compute_stream, int hold,
+                        uint64_t* ticket);
+/* Once `ticket` has drained (FC_ENOTREADY before): the bytes its drain moved and
+ * whether it was an incremental save (1) or a full one (0). */
+int fc_save_delta_stats(fc_ctx* ctx, uint64_t ticket, uint64_t* drained_bytes, int* delta);
+/* Forget the baseline: the next fc_save_delta_async is a full save. */
+int fc_delta_invalidate(fc_ctx* ctx);
+
 /* FC_OK once nothing of save `ticket` reads the source tensors any more (they may
  * change): its gather kernel, if any, has finished and its in-place part, if any,
  * has been drained; FC_ENOTREADY before.  fc_save_sources_wait blocks the calling
