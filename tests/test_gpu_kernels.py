@@ -52,16 +52,24 @@ def test_pack_matches_oracle(cuda_device, variant, aligned, chunk):
     ctx = native.get_context(0)
     tensors, offsets, total = _ragged_case(1, aligned)
     ctx.arena_reserve(total)
+    size = min(ctx.arena_info()[1], total + 4096)  # the shared arena may be far larger
+    # canary: the gaps between ranges (aligned case) and the bytes past the last range
+    # must keep what they held
+    canary = ((np.arange(size) * 131 + 7) & 255).astype(np.uint8)
+    ctx.arena_tensor(size).copy_(torch.from_numpy(canary))
     plan = ctx.plan([t.data_ptr() for t in tensors], offsets, [t.numel() for t in tensors], chunk)
     assert plan.payload_bytes == sum(t.numel() for t in tensors)
     plan.pack(torch.cuda.current_stream(), variant)
     torch.cuda.synchronize()
-    got = _arena_bytes(ctx, total)
-    want = oracle.pack_ranges([oracle.tensor_bytes(t) for t in tensors], offsets, total)
-    # gaps (aligned case) are don't-care: compare only covered bytes
+    got = _arena_bytes(ctx, size)
+    want = canary.copy()
+    for t, o in zip(tensors, offsets):
+        want[o:o + t.numel()] = oracle.tensor_bytes(t)
     for t, o in zip(tensors, offsets):
         n = t.numel()
         assert np.array_equal(got[o:o + n], want[o:o + n]), f"range at {o} len {n}"
+    bad = np.flatnonzero(got != want)
+    assert bad.size == 0, f"bytes outside the ranges written at {bad[:8]}"
     plan.destroy()
 
 

@@ -18,6 +18,7 @@ from dlrover_b200 import _native as native
 from dlrover_b200.shm_handler import (DLROVER_CKPT_CONFIG_KEY, CheckpointConfig,
                                       SharedMemoryHandler, _DeviceStager)
 from oracle import shm_layout as oracle
+from tests import plan_model as pm
 
 CHUNK = 64 << 10
 gpu = pytest.mark.gpu
@@ -76,6 +77,14 @@ def _check(host, ctx, leaves, offsets, total):
         assert np.array_equal(arena[o:o + t.numel()], want[o:o + t.numel()]), "arena"
 
 
+def _drained(leaves, offsets, total, old):
+    """The bytes an incremental save must drain: the items (CHUNK plan) in which the
+    oracle image of the current tensors differs from `old`."""
+    its = pm.items([pm.Range(t.data_ptr(), o, t.numel()) for t, o in zip(leaves, offsets)],
+                   CHUNK)
+    return pm.drained_bytes(pm.dirty(its, old, _want(leaves, offsets, total)))
+
+
 def _save(ctx, plan, host_addr, **kw):
     ticket = plan.save_delta_async(host_addr, torch.cuda.current_stream(), **kw)
     ctx.save_wait(ticket)
@@ -116,19 +125,22 @@ def test_delta_parity_through_the_c_abi(cuda_device, variant):
                (headed, 0), (headed, 8), (headed, 100_000), (headed, headed.numel() - 1),
                (tiny, 4), (last, last.numel() - 1)]      # the last byte of the plan
     for t, i in changes:
+        old = _want(leaves, offsets, total)
         _bump(t, i)
         delta, n = _save(ctx, plan, addr)
-        assert delta and 1 <= n <= CHUNK, (i, n)
+        assert delta and n == _drained(leaves, offsets, total, old), (i, n)
         _check(hnp, ctx, leaves, offsets, total)
+    old = _want(leaves, offsets, total)
     for t, i in changes:  # all at once
         _bump(t, i)
     delta, n = _save(ctx, plan, addr)
-    assert delta and len(changes) <= n <= len(changes) * CHUNK
+    assert delta and n == _drained(leaves, offsets, total, old)
     _check(hnp, ctx, leaves, offsets, total)
 
+    old = _want(leaves, offsets, total)
     shifted.copy_(torch.randint(0, 256, shifted.shape, dtype=torch.uint8, device="cuda"))
     delta, n = _save(ctx, plan, addr)  # one leaf rewritten
-    assert delta and shifted.numel() <= n <= shifted.numel() + 2 * CHUNK
+    assert delta and n == _drained(leaves, offsets, total, old)
     _check(hnp, ctx, leaves, offsets, total)
 
     for t in leaves:  # every item, one byte or two each
@@ -241,10 +253,11 @@ def test_staged_and_sliced_drain_of_dirty_runs(cuda_device):
 
         assert _save(ctx, plan, seg.addr)[0] is False  # pageable: bounce slots
         _check(hnp, ctx, leaves, offsets, total)
+        old = _want(leaves, offsets, total)
         for off in (100, (3 << 20) + 7, total - 1):
             _bump(*at(off))
         delta, n = _save(ctx, plan, seg.addr)
-        assert delta and 3 <= n <= 3 * CHUNK
+        assert delta and n == _drained(leaves, offsets, total, old)
         _check(hnp, ctx, leaves, offsets, total)
 
         ctx.host_register_background(seg.addr, total, slice_bytes=4 << 20)
@@ -257,6 +270,7 @@ def test_staged_and_sliced_drain_of_dirty_runs(cuda_device):
             ctx.set_drain_mode(mode)
             # dirty items on both sides of the 4 MiB and 8 MiB slice boundaries: their
             # merged runs straddle a slice, so the drain must cut them there
+            old = _want(leaves, offsets, total)
             for off in range((4 << 20) - 2 * CHUNK, (4 << 20) + 2 * CHUNK, CHUNK // 2):
                 _bump(*at(off))
             for off in ((8 << 20) - 10, (8 << 20) + 10):
@@ -264,7 +278,7 @@ def test_staged_and_sliced_drain_of_dirty_runs(cuda_device):
             _, m0 = ctx.launch_count()
             delta, n = _save(ctx, plan, seg.addr)
             _, m1 = ctx.launch_count()
-            assert delta and 4 * CHUNK <= n <= 8 * CHUNK
+            assert delta and n == _drained(leaves, offsets, total, old)
             assert m1 - m0 >= 4  # two runs, each cut at a slice boundary
             _check(hnp, ctx, leaves, offsets, total)
         ctx.host_unregister(seg.addr)
