@@ -22,6 +22,7 @@ FC_EINVAL = -1
 FC_ECUDA = -2
 FC_ENOMEM = -3
 FC_EBUSY = -4
+FC_ENOIMAGE = -5
 FC_ENOTREADY = 1
 
 VARIANT_AUTO = 0
@@ -116,6 +117,8 @@ _SIGNATURES = {
     "fc_arena_fill": (ctypes.c_int, [_vp, _vp, _u64, _u64, _vp]),
     "fc_restore_wait": (ctypes.c_int, [_vp]),
     "fc_restore_timings": (ctypes.c_int, [_vp, _fp, _fp, _fp]),
+    "fc_restore_from_image_async": (ctypes.c_int, [_vp, _vp, _vp]),
+    "fc_image_covers": (ctypes.c_int, [_vp, _vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
@@ -298,6 +301,27 @@ class Plan:
         else:
             _check(lib.fc_restore_async(self.handle, host_ptr, _stream_ptr(stream)),
                    "fc_restore_async")
+
+    def restore_from_image_async(self, host_ptr: int, stream=None) -> bool:
+        """Rollback: scatter the arena image of the last drained full-arena save into the
+        plan's tensors (no DMA); Context.restore_wait applies.  False when the arena holds
+        no image covering this plan for `host_ptr` (nothing enqueued: restore from host
+        memory instead)."""
+        rc = load_library().fc_restore_from_image_async(self.handle, host_ptr,
+                                                        _stream_ptr(stream))
+        if rc == FC_ENOIMAGE:
+            return False
+        _check(rc, "fc_restore_from_image_async")
+        return True
+
+    def image_covers(self, host_ptr: int) -> bool:
+        """Whether restore_from_image_async would find an image covering this plan (no
+        side effect)."""
+        rc = load_library().fc_image_covers(self.handle, host_ptr)
+        if rc == FC_ENOIMAGE:
+            return False
+        _check(rc, "fc_image_covers")
+        return True
 
     def destroy(self):
         if self._h:

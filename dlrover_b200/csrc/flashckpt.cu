@@ -83,6 +83,7 @@ extern "C" const char* fc_strerror(int code) {
     case FC_ECUDA: return "CUDA runtime error";
     case FC_ENOMEM: return "out of memory";
     case FC_EBUSY: return "a save/restore is still in flight";
+    case FC_ENOIMAGE: return "the arena holds no image of the segment for this plan";
     case FC_ENOTREADY: return "not ready";
     default: return "unknown flashckpt error";
   }
@@ -201,6 +202,15 @@ struct fc_ctx {
   const uint8_t* base_host = nullptr;
   bool base_valid = false;
   uint64_t base_ticket = 0;  // the delta save that becomes the baseline once drained
+  // Arena image (fc_restore_from_image_async): for every run of img_map, arena byte `off`
+  // equals segment byte `hoff` at img_host.  Set by a full-arena fc_save_async* or an
+  // fc_save_delta_async once it has drained without error, kept by the rollback, forgotten
+  // by everything that forgets the baseline.  Guarded by `mu`.
+  std::shared_ptr<const DeltaMap> img_map;
+  const fc_plan* img_plan = nullptr;
+  const uint8_t* img_host = nullptr;
+  bool img_valid = false;
+  uint64_t img_ticket = 0;  // the save that sets the image once drained
   // dirty marks: one entry per `all` item of the plan being saved, = the save's seq
   uint32_t* dirty = nullptr;
   uint32_t* dirty_pinned = nullptr;
@@ -211,10 +221,27 @@ struct fc_ctx {
   int stat_delta = 0;
 };
 
-static void delta_forget_locked(fc_ctx* c) {
+static void baseline_forget_locked(fc_ctx* c) {
   c->base_valid = false;
   c->base_ticket = 0;
 }
+
+static void image_forget_locked(fc_ctx* c) {
+  c->img_valid = false;
+  c->img_ticket = 0;
+}
+
+// The arena or the segment may no longer hold the image: forget the incremental baseline
+// and the arena image.
+static void delta_forget_locked(fc_ctx* c) {
+  baseline_forget_locked(c);
+  image_forget_locked(c);
+}
+
+// A save that leaves the arena a byte image of the segment for plan p (full-arena gather,
+// then a drain of every run it changed): the image is valid once ticket has drained.
+static void image_expect_locked(fc_ctx* c, const fc_plan* p, const uint8_t* host,
+                                uint64_t ticket);
 
 static void delta_forget(fc_ctx* c) {
   std::lock_guard<std::mutex> lk(c->mu);
@@ -504,8 +531,10 @@ static void pump_main(fc_ctx* c) {
         c->drain_err = std::string("drain pump: ") + cudaGetErrorString(e);
         (void)cudaGetLastError();
         delta_forget_locked(c);
-      } else if (job.ticket == c->base_ticket) {
-        c->base_valid = true;  // the segment now holds the arena's image of this plan
+      } else {
+        // the segment now holds the arena's image of this plan
+        if (job.ticket == c->base_ticket) c->base_valid = true;
+        if (job.ticket == c->img_ticket) c->img_valid = true;
       }
       c->stat_ticket = job.ticket;
       c->stat_bytes = drained;
@@ -550,6 +579,15 @@ struct fc_plan {
   cudaEvent_t ev_upload = nullptr;  // last table upload
   cudaEvent_t ev_last_use = nullptr;  // last kernel that read the tables
 };
+
+static void image_expect_locked(fc_ctx* c, const fc_plan* p, const uint8_t* host,
+                                uint64_t ticket) {
+  c->img_map = p->dmap;
+  c->img_plan = p;
+  c->img_host = host;
+  c->img_valid = false;
+  c->img_ticket = ticket;
+}
 
 struct DeviceGuard {
   int prev = -1;
@@ -1210,7 +1248,8 @@ static int plan_fill(fc_plan* p, uint32_t n, const void* const* dev_ptrs,
   // that moves a byte of the image does not
   if (!p->dmap || !p->dmap->same_extents(*dmap)) {
     std::lock_guard<std::mutex> lk(c->mu);
-    if (c->base_plan == p) delta_forget_locked(c);
+    if (c->base_plan == p) baseline_forget_locked(c);
+    if (c->img_plan == p) image_forget_locked(c);
   }
   p->dmap = std::move(dmap);
   p->runs.swap(runs);
@@ -1323,8 +1362,13 @@ extern "C" int fc_plan_destroy(fc_plan* p) {
   {
     std::lock_guard<std::mutex> lk(c->mu);
     if (c->base_plan == p) {
-      delta_forget_locked(c);
+      baseline_forget_locked(c);
       c->base_plan = nullptr;  // a later plan may be allocated at the same address
+    }
+    if (c->img_plan == p) {
+      image_forget_locked(c);
+      c->img_plan = nullptr;
+      c->img_map.reset();
     }
   }
   for (FcTable* t : {&p->all, &p->bulk, &p->resid, &p->shift}) {
@@ -1687,6 +1731,7 @@ static int save_async_impl(fc_plan* p, void* host_base, void* compute_stream, ui
     if (hold) c->held_ticket = c->ticket;
     c->jobs.push_back(std::move(job));
     c->save_inflight = true;
+    image_expect_locked(c, p, static_cast<uint8_t*>(host_base), c->ticket);
     if (ticket) *ticket = c->ticket;
   }
   c->cv.notify_all();
@@ -1905,6 +1950,7 @@ extern "C" int fc_save_delta_async(fc_plan* p, void* host_base, void* compute_st
     c->base_plan = p;
     c->base_host = host;
     c->base_ticket = c->ticket;
+    image_expect_locked(c, p, host, c->ticket);
     if (ticket) *ticket = c->ticket;
   }
   c->cv.notify_all();
@@ -2249,6 +2295,63 @@ extern "C" int fc_restore_async(fc_plan* p, const void* host_base, void* stream)
   FC_CUDA(cudaStreamWaitEvent(s, c->ev_fill_end, 0));
   rc = launch_copy<1>(p, s, FC_VARIANT_AUTO);
   if (rc) return rc;
+  FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
+  c->restore_inflight = true;
+  return FC_OK;
+}
+
+// ---- rollback from the arena image ----------------------------------------------
+// Every run of `p`, as (arena off, segment hoff, len), must lie inside one run of the
+// image map at the same offset on both sides: then the arena holds, at p's arena offsets,
+// exactly the bytes fc_restore_async would fetch from host_base.  The image runs are
+// sorted by arena offset and do not overlap: one binary search per run of p.
+static bool image_covers_locked(const fc_ctx* c, const fc_plan* p, const uint8_t* host) {
+  if (!c->img_valid || !c->img_map || c->img_host != host) return false;
+  if (p->arena_end > c->arena_bytes) return false;
+  const std::vector<FcRun>& img = c->img_map->runs;
+  for (const FcRun& r : p->runs) {
+    auto it = std::upper_bound(img.begin(), img.end(), r.off,
+                               [](uint64_t v, const FcRun& m) { return v < m.off; });
+    if (it == img.begin()) return false;
+    const FcRun& m = *(it - 1);
+    const uint64_t in = r.off - m.off;
+    if (in + r.len > m.len || r.hoff < m.hoff || r.hoff - m.hoff != in) return false;
+  }
+  return true;
+}
+
+extern "C" int fc_image_covers(const fc_plan* p, const void* host_base) {
+  if (!p || (!host_base && p->payload)) return fail(FC_EINVAL, "fc_image_covers: null argument%s%s");
+  fc_ctx* c = p->ctx;
+  std::lock_guard<std::mutex> lk(c->mu);
+  return image_covers_locked(c, p, static_cast<const uint8_t*>(host_base)) ? FC_OK : FC_ENOIMAGE;
+}
+
+extern "C" int fc_restore_from_image_async(fc_plan* p, const void* host_base, void* stream) {
+  if (!p || (!host_base && p->payload))
+    return fail(FC_EINVAL, "fc_restore_from_image_async: null argument%s%s");
+  fc_ctx* c = p->ctx;
+  FC_GUARD(c);
+  int rc = refresh_inflight(c);
+  if (rc) return rc;
+  if (c->save_inflight || c->restore_inflight)
+    return fail(FC_EBUSY, "fc_restore_from_image_async: context busy%s%s");
+  {
+    // nothing runs between this check and the scatter's enqueue that could change the
+    // record: saves, restores and plan updates of this context refuse while it is busy,
+    // and the pump has drained every ticket (save_inflight is false)
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (!image_covers_locked(c, p, static_cast<const uint8_t*>(host_base)))
+      return fail(FC_ENOIMAGE, "fc_restore_from_image_async: no arena image covers the plan%s%s");
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  // no fill: both fill events on `stream`, so fc_restore_timings reports fill 0 and the
+  // scatter alone
+  FC_CUDA(cudaEventRecord(c->ev_fill_start, s));
+  FC_CUDA(cudaEventRecord(c->ev_fill_end, s));
+  rc = launch_copy<1>(p, s, FC_VARIANT_AUTO);
+  if (rc) return rc;
+  // the next save, restore or fill refuses (FC_EBUSY) until the scatter has read the arena
   FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
   c->restore_inflight = true;
   return FC_OK;

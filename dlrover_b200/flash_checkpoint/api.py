@@ -111,6 +111,16 @@ class DdpCheckpointer(Checkpointer):
                                          stream=stream, strict=strict)
         return step
 
+    def rollback_into(self, state_dict, stream=None, strict=True):
+        """Roll the live tensors of `state_dict` back to the in-memory checkpoint this
+        process saved: from the HBM snapshot of that save when every rank still holds
+        it (no PCIe transfer, the incremental baseline survives), else exactly as
+        load_checkpoint_into.  Returns the restored step, 0 if memory holds nothing
+        usable."""
+        step, _ = self._engine.rollback_into({CheckpointConstant.MODEL_STATES_NAME: state_dict},
+                                             stream=stream, strict=strict)
+        return step
+
     def wait_memory_save(self, timeout=None):
         """Block until the last save_checkpoint(MEMORY) is fully in shared memory."""
         return self._engine.wait_memory_save(timeout)

@@ -21,6 +21,8 @@ Behavioural differences, all on the device path:
   * the readiness all-reduce runs on a side stream and only that stream is
     synchronised, so the check no longer waits for the training stream.
   * load_into(): scatter the in-memory checkpoint straight into live tensors.
+  * rollback_into(): the same from the HBM snapshot of this process's last save
+    when every rank still holds one (no PCIe transfer).
 """
 
 from __future__ import annotations
@@ -786,6 +788,31 @@ class CheckpointEngine(metaclass=ABCMeta):
         stats = self._shm_handler.restore_into(target_state_dict, stream=stream, strict=strict,
                                                pin_after=not self._coop_wanted, coop=coop)
         return config.step, stats
+
+    def rollback_into(self, target_state_dict, stream=None, strict=True):
+        """load_into for a process that saved the in-memory checkpoint itself (a rollback
+        after a loss spike, or a survivor resetting to the last consistent step): when
+        every rank of the loader group still holds the arena image of its last memory
+        save, each rank scatters from HBM and nothing crosses PCIe; the incremental
+        baseline survives.  If any rank holds none, every rank takes the load_into path
+        (its cooperative restore needs all local ranks in one all-gather).  Returns
+        (step, stats); stats["from_image"] says which path ran."""
+        config = self._shm_handler.get_checkpoint_config(CheckpointConfig())
+        passed = verify_all_rank_step_consistent(self._loader_group, config.step)
+        image = False
+        if passed and config.step > 0:
+            try:
+                image = self._shm_handler.can_rollback(target_state_dict, strict=strict)
+            except Exception:
+                image = False  # load_into below raises the same error on this rank
+        if all_reduce_flags(self._loader_group, [0 if image else 1])[0] == 0:
+            stats = self._shm_handler.rollback_into(target_state_dict, stream=stream,
+                                                    strict=strict)
+            return config.step, stats
+        step, stats = self.load_into(target_state_dict, stream=stream, strict=strict)
+        if stats:
+            stats["from_image"] = 0.0
+        return step, stats
 
     def _restore_memory_from_replica(self):
         if not self._replica_manager.has_replica():

@@ -1494,6 +1494,55 @@ class SharedMemoryHandler:
         restore at the same time — each rank reads only 1/n of the image from host
         memory into its arena and the slices are exchanged over NVLink (NCCL
         all-gather, in place) before the scatter kernel; every rank must call."""
+        device_pairs, host_pairs = self._restore_targets(target, strict)
+        stats = {"device_bytes": 0.0, "host_bytes": 0.0, "fill_ms": 0.0, "scatter_ms": 0.0}
+        with torch.no_grad():
+            stats["host_bytes"] = self._restore_host_leaves(host_pairs)
+            if device_pairs:
+                stager, plan, stream = self._restore_plan(device_pairs, stream)
+                if coop is not None:
+                    stats.update(self._run_restore_cooperative(stager, plan, stream, coop))
+                else:
+                    stats.update(self._run_restore(stager, plan, stream, pin_after=pin_after))
+        return stats
+
+    def rollback_into(self, target, stream=None, strict: bool = True) -> Dict[str, float]:
+        """restore_into for a process that saved the checkpoint itself: after a
+        full-snapshot save has drained, the HBM arena still holds the image of what it
+        wrote, and the CUDA leaves are scattered from there (one scatter kernel, nothing
+        crosses PCIe).  The incremental baseline survives, so the next incremental save
+        drains only what changed after the rollback.  Without such an image (in-place,
+        hybrid, bounded-arena or cooperative saves, a restore or anything else that
+        rewrote the arena since) this is restore_into.  CPU leaves come from the segment
+        either way.  stats: those of restore_into plus "from_image" (1.0 / 0.0)."""
+        device_pairs, host_pairs = self._restore_targets(target, strict)
+        stats = {"device_bytes": 0.0, "host_bytes": 0.0, "fill_ms": 0.0, "scatter_ms": 0.0,
+                 "from_image": 0.0}
+        with torch.no_grad():
+            stats["host_bytes"] = self._restore_host_leaves(host_pairs)
+            if device_pairs:
+                stager, plan, stream = self._restore_plan(device_pairs, stream)
+                got = self._run_rollback(stager, plan, stream)
+                if got is None:
+                    got = self._run_restore(stager, plan, stream)
+                    got["from_image"] = self.last_restore_stats["from_image"] = 0.0
+                stats.update(got)
+        return stats
+
+    def can_rollback(self, target, strict: bool = True) -> bool:
+        """Whether rollback_into(target) would scatter every CUDA leaf from the arena
+        image; restores nothing.  False when the tree has no CUDA leaf."""
+        device_pairs, _ = self._restore_targets(target, strict)
+        if not device_pairs:
+            return False
+        _, plan, _ = self._restore_plan(device_pairs, None)
+        return plan.image_covers(self.shared_memory.dma_address)
+
+    def _restore_targets(self, target, strict: bool):
+        """The part every restore of the in-memory checkpoint into live tensors shares:
+        wait for this handler's own drain, refuse a checkpoint that is being written, map
+        the segment, and pair each tensor leaf of `target` with its meta (tree, strictness,
+        shape and dtype checks).  Returns (CUDA pairs, CPU pairs)."""
         self.wait_pending()
         meta_dict = self.metadata.get()
         config = meta_dict.get(DLROVER_CKPT_CONFIG_KEY, CheckpointConfig())
@@ -1538,32 +1587,46 @@ class SharedMemoryHandler:
                     (device_pairs if tgt.is_cuda else host_pairs).append((tgt, meta))
 
         walk(target, meta_dict, "")
-        stats = {"device_bytes": 0.0, "host_bytes": 0.0, "fill_ms": 0.0, "scatter_ms": 0.0}
-        with torch.no_grad():
-            strided = [(t, m) for t, m in host_pairs if not t.is_contiguous()]
-            dense = [(t, m) for t, m in host_pairs if t.is_contiguous()]
-            for t, m in strided:  # rare: let torch handle the strides
-                t.copy_(_read_tensor_from_buf(m, self.shared_memory))
-            if dense:
-                native.host_unpack(self.shared_memory.address, [t.data_ptr() for t, _ in dense],
-                                   [m.offset for _, m in dense],
-                                   [m.numel * m.element_size for _, m in dense], _host_threads())
-            stats["host_bytes"] = float(sum(m.numel * m.element_size for _, m in host_pairs))
-            if device_pairs:
-                stager = self._stager_for([t for t, _ in device_pairs])
-                prepared = stager.prepare_ranges(
-                    [(t, m.offset, m.numel * m.element_size) for t, m in device_pairs], [],
-                    for_write=True)
-                if stager._attached is None:
-                    stager.attach(self.shared_memory)
-                if stream is None:
-                    stream = torch.cuda.current_stream(stager.device_index)
-                plan = stager.plan_for(prepared, role="restore", stream=stream)
-                if coop is not None:
-                    stats.update(self._run_restore_cooperative(stager, plan, stream, coop))
-                else:
-                    stats.update(self._run_restore(stager, plan, stream, pin_after=pin_after))
-        return stats
+        return device_pairs, host_pairs
+
+    def _restore_host_leaves(self, host_pairs) -> float:
+        """CPU leaves straight from the segment; returns their bytes."""
+        strided = [(t, m) for t, m in host_pairs if not t.is_contiguous()]
+        dense = [(t, m) for t, m in host_pairs if t.is_contiguous()]
+        for t, m in strided:  # rare: let torch handle the strides
+            t.copy_(_read_tensor_from_buf(m, self.shared_memory))
+        if dense:
+            native.host_unpack(self.shared_memory.address, [t.data_ptr() for t, _ in dense],
+                               [m.offset for _, m in dense],
+                               [m.numel * m.element_size for _, m in dense], _host_threads())
+        return float(sum(m.numel * m.element_size for _, m in host_pairs))
+
+    def _restore_plan(self, device_pairs, stream):
+        """(stager, restore plan, stream) for the CUDA leaves: arena offset = segment
+        offset of every leaf, so the plan lines up with the saves' arena image."""
+        stager = self._stager_for([t for t, _ in device_pairs])
+        prepared = stager.prepare_ranges(
+            [(t, m.offset, m.numel * m.element_size) for t, m in device_pairs], [],
+            for_write=True)
+        if stager._attached is None:
+            stager.attach(self.shared_memory)
+        if stream is None:
+            stream = torch.cuda.current_stream(stager.device_index)
+        plan = stager.plan_for(prepared, role="restore", stream=stream)
+        return stager, plan, stream
+
+    def _run_rollback(self, stager: _DeviceStager, plan, stream) -> Optional[Dict[str, float]]:
+        """One scatter kernel from the arena image; None (nothing done) without one."""
+        t0 = time.perf_counter()
+        if not plan.restore_from_image_async(self.shared_memory.dma_address, stream):
+            return None
+        stager.ctx.restore_wait()
+        wall_ms = (time.perf_counter() - t0) * 1e3
+        _, scatter, _ = stager.ctx.restore_timings()
+        self.last_restore_stats = {"device_bytes": float(plan.payload_bytes), "fill_ms": 0.0,
+                                   "scatter_ms": scatter, "direct": 0.0, "staged": 0.0,
+                                   "wall_ms": wall_ms, "from_image": 1.0}
+        return dict(self.last_restore_stats)
 
     def _run_restore_cooperative(self, stager: _DeviceStager, plan, stream, coop):
         """Each of the n local ranks fills 1/n of its arena from the segment (its own PCIe

@@ -47,6 +47,7 @@ enum {
   FC_ECUDA = -2,   /* a CUDA runtime call failed; see fc_last_error()            */
   FC_ENOMEM = -3,  /* host or device allocation failed                           */
   FC_EBUSY = -4,   /* a save/restore is still in flight on this context          */
+  FC_ENOIMAGE = -5, /* the arena holds no image of the segment for this plan     */
   FC_ENOTREADY = 1 /* poll: work still pending (not an error)                    */
 };
 
@@ -249,7 +250,8 @@ int fc_save_delta_async(fc_plan* plan, void* host_base, void* compute_stream, in
 /* Once `ticket` has drained (FC_ENOTREADY before): the bytes its drain moved and
  * whether it was an incremental save (1) or a full one (0). */
 int fc_save_delta_stats(fc_ctx* ctx, uint64_t ticket, uint64_t* drained_bytes, int* delta);
-/* Forget the baseline: the next fc_save_delta_async is a full save. */
+/* Forget the baseline (the next fc_save_delta_async is a full save) and the arena image
+ * (the next fc_restore_from_image_async answers FC_ENOIMAGE). */
 int fc_delta_invalidate(fc_ctx* ctx);
 
 /* FC_OK once nothing of save `ticket` reads the source tensors any more (they may
@@ -322,6 +324,33 @@ int fc_restore_direct_async(fc_plan* plan, const void* host_base, void* stream);
 int fc_arena_fill(fc_ctx* ctx, const void* host_base, uint64_t lo, uint64_t hi, void* stream);
 int fc_restore_wait(fc_ctx* ctx);
 int fc_restore_timings(fc_ctx* ctx, float* fill_ms, float* scatter_ms, float* total_ms);
+
+/* ---- rollback: restore from the arena image ------------------------------- */
+
+/* After a save has drained, the arena still holds a byte image of what it wrote to the
+ * segment.  The context records it: the plan's runs (arena offset -> segment offset) and
+ * host_base of the last full-arena fc_save_async / fc_save_async_held or
+ * fc_save_delta_async (full or incremental) that drained without error.  A rollback keeps
+ * the record, and so does an fc_plan_update* that only re-targets the tensor pointers of
+ * that plan.  Every event that forgets the incremental baseline forgets it too (the other
+ * saves, every restore, pack / unpack, fc_arena_fill, arena reallocation, fc_save_cancel,
+ * a drain error, fc_plan_destroy of that plan, an update that moves a range,
+ * fc_delta_invalidate).  Bounded-arena, in-place and hybrid saves never set it.
+ *
+ * Restore from the arena image: if the context's arena holds, for host_base, the bytes
+ * every range of `plan` restores from, enqueue the scatter arena -> tensors on `stream`
+ * (the plan's unpack kernels, no DMA) and return FC_OK; fc_restore_wait /
+ * fc_restore_timings apply (fill 0).  FC_ENOIMAGE when there is no image or it does not
+ * cover the plan: nothing is enqueued, nothing is forgotten, the caller restores from
+ * host memory.  FC_EBUSY while a save/restore is in flight.  Keeps the image and the
+ * incremental baseline.
+ * Coverage: every run of `plan`, as (arena offset, segment offset, length), lies inside
+ * one run of the image at the same offset into that run on both sides.  A restore plan
+ * over a subset of the saved ranges is covered. */
+int fc_restore_from_image_async(fc_plan* plan, const void* host_base, void* stream);
+/* The coverage test alone, nothing enqueued: FC_OK when the image covers `plan` for
+ * host_base, FC_ENOIMAGE when not (also while the save that would set it has not drained). */
+int fc_image_covers(const fc_plan* plan, const void* host_base);
 
 #ifdef __cplusplus
 }
