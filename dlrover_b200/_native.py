@@ -29,6 +29,15 @@ VARIANT_AUTO = 0
 VARIANT_LSU = 1
 VARIANT_TMA = 2
 
+# element kinds of the non-finite scan (FC_KIND_*)
+KIND_NONE = 0
+KIND_F16 = 1
+KIND_BF16 = 2
+KIND_F32 = 3
+KIND_F64 = 4
+KIND_E5M2 = 5
+KIND_E4M3FN = 6
+
 DRAIN_HOST_PACED = 0
 DRAIN_PINGPONG = 1
 
@@ -119,6 +128,9 @@ _SIGNATURES = {
     "fc_restore_timings": (ctypes.c_int, [_vp, _fp, _fp, _fp]),
     "fc_restore_from_image_async": (ctypes.c_int, [_vp, _vp, _vp]),
     "fc_image_covers": (ctypes.c_int, [_vp, _vp]),
+    "fc_plan_set_kinds": (ctypes.c_int, [_vp, _u32, ctypes.POINTER(ctypes.c_uint8)]),
+    "fc_scan_nonfinite_async": (ctypes.c_int, [_vp, _vp]),
+    "fc_scan_wait": (ctypes.c_int, [_vp, ctypes.POINTER(_u64), ctypes.POINTER(_u32), _u32]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
@@ -322,6 +334,27 @@ class Plan:
             return False
         _check(rc, "fc_image_covers")
         return True
+
+    def set_kinds(self, kinds: Sequence[int]):
+        """One KIND_* per range of the last create / update (empty ranges included); kept
+        across updates with the same number of ranges."""
+        n = len(kinds)
+        arr = (ctypes.c_uint8 * max(n, 1))(*[int(k) for k in kinds])
+        _check(load_library().fc_plan_set_kinds(self.handle, n, arr), "fc_plan_set_kinds")
+
+    def scan_nonfinite_async(self, stream=None):
+        """Enqueue on `stream` the count of NaN / Inf elements of every range (read-only;
+        see scan_wait)."""
+        _check(load_library().fc_scan_nonfinite_async(self.handle, _stream_ptr(stream)),
+               "fc_scan_nonfinite_async")
+
+    def scan_wait(self, n_ranges: int) -> Tuple[int, list]:
+        """(total, per-range counts) of the last scan, once it has finished."""
+        total = _u64()
+        counts = (_u32 * max(n_ranges, 1))()
+        _check(load_library().fc_scan_wait(self.handle, ctypes.byref(total), counts, n_ranges),
+               "fc_scan_wait")
+        return total.value, list(counts[:n_ranges])
 
     def destroy(self):
         if self._h:

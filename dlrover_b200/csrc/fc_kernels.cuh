@@ -667,3 +667,107 @@ fc_delta_tma(const FcItem* __restrict__ items, uint32_t n_items, uint8_t* __rest
   }
   if (threadIdx.x == 0) bulk_wait_all();
 }
+
+// ------------------------------------------------------------- non-finite scan --
+// fc_scan_nonfinite: read-only scan of the source bytes of a plan that counts the
+// elements whose exponent field is all ones (NaN or +-Inf).  float8_e4m3fn has no Inf:
+// only its NaN patterns (0x7F, 0xFF) count.  Complex kinds are scanned as their float
+// components.  Its own item table: FcItem.tptr = element-aligned source address,
+// .nbytes = whole elements (<= kDefaultChunk), .aoff = kind (FC_KIND_*), .pad0 = index of
+// the input range.  Bodies: 128-bit non-allocating loads, 4x unrolled as in copy_range;
+// 16-B heads and tails: element loads.  Traffic: 1 byte read per scanned byte; clean
+// data writes nothing, an item with a hit costs one atomic per warp per output.
+enum : uint32_t {
+  kScanF16 = 1,
+  kScanBF16 = 2,
+  kScanF32 = 3,
+  kScanF64 = 4,
+  kScanE5M2 = 5,
+  kScanE4M3 = 6
+};
+
+// hits in one 32-bit word (F64: the word holding an element's exponent)
+template <uint32_t K>
+__device__ __forceinline__ uint32_t bad_word(uint32_t w) {
+  if (K == kScanF64) return (w & 0x7FF00000u) == 0x7FF00000u;
+  if (K == kScanF32) return (w & 0x7F800000u) == 0x7F800000u;
+  if (K == kScanF16) return __popc(__vcmpeq2(w & 0x7C007C00u, 0x7C007C00u)) >> 4;
+  if (K == kScanBF16) return __popc(__vcmpeq2(w & 0x7F807F80u, 0x7F807F80u)) >> 4;
+  if (K == kScanE5M2) return __popc(__vcmpeq4(w & 0x7C7C7C7Cu, 0x7C7C7C7Cu)) >> 3;
+  return __popc(__vcmpeq4(w & 0x7F7F7F7Fu, 0x7F7F7F7Fu)) >> 3;  // e4m3fn: S.1111.111
+}
+
+template <uint32_t K>
+__device__ __forceinline__ uint32_t bad_vec(const uint4& v) {
+  // a 16-B aligned vector holds whole elements; a float64's exponent is in its high word
+  if (K == kScanF64) return bad_word<K>(v.y) + bad_word<K>(v.w);
+  return bad_word<K>(v.x) + bad_word<K>(v.y) + bad_word<K>(v.z) + bad_word<K>(v.w);
+}
+
+// one element of ES bytes, zero-extended (the upper lanes of the word then never match)
+template <uint32_t K, uint32_t ES>
+__device__ __forceinline__ uint32_t bad_elem(const uint8_t* p) {
+  if (ES == 8) return bad_word<K>(__ldg(reinterpret_cast<const uint32_t*>(p) + 1));
+  if (ES == 4) return bad_word<K>(__ldg(reinterpret_cast<const uint32_t*>(p)));
+  if (ES == 2) return bad_word<K>(__ldg(reinterpret_cast<const unsigned short*>(p)));
+  return bad_word<K>(__ldg(reinterpret_cast<const unsigned char*>(p)));
+}
+
+// this thread's hits among the n bytes at p (p and n multiples of ES)
+template <uint32_t K, uint32_t ES>
+__device__ __forceinline__ uint32_t scan_range(const uint8_t* __restrict__ p, uint32_t n) {
+  constexpr int T = kLsuThreads, U = kLsuUnroll;
+  uint32_t head = (uint32_t)((16u - ((uintptr_t)p & 15u)) & 15u);
+  if (head > n) head = n;
+  const uint32_t body = (n - head) & ~15u;
+  const uint32_t nhead = head / ES, ntail = (n - head - body) / ES;
+  uint32_t bad = 0;
+  if (threadIdx.x < nhead)
+    bad += bad_elem<K, ES>(p + threadIdx.x * ES);
+  else if (threadIdx.x < nhead + ntail)
+    bad += bad_elem<K, ES>(p + head + body + (threadIdx.x - nhead) * ES);
+  const uint4* __restrict__ s = reinterpret_cast<const uint4*>(p + head);
+  const uint32_t nvec = body >> 4;
+  uint32_t i = threadIdx.x;
+  for (; i + (U - 1) * T < nvec; i += U * T) {
+    uint4 v[U];
+#pragma unroll
+    for (int j = 0; j < U; ++j) v[j] = ldg_stream(s + i + j * T);
+#pragma unroll
+    for (int j = 0; j < U; ++j) bad += bad_vec<K>(v[j]);
+  }
+  for (; i < nvec; i += T) bad += bad_vec<K>(ldg_stream(s + i));
+  return bad;
+}
+
+__device__ __forceinline__ void add_saturating(uint32_t* c, uint32_t v) {
+  const uint32_t old = atomicAdd(c, v);
+  if (old + v < old) atomicMax(c, 0xFFFFFFFFu);  // every wrap is followed by its own max
+}
+
+// counts[range] += hits of the item (saturating), *total += hits.
+__global__ void __launch_bounds__(kLsuThreads)
+fc_scan_nonfinite(const FcItem* __restrict__ items, uint32_t n_items, uint32_t* counts,
+                  unsigned long long* total) {
+  for (uint32_t c = blockIdx.x; c < n_items; c += gridDim.x) {
+    const uint4 a = __ldg(reinterpret_cast<const uint4*>(items + c));
+    const uint4 b = __ldg(reinterpret_cast<const uint4*>(items + c) + 1);
+    const uint8_t* p = reinterpret_cast<const uint8_t*>(((uint64_t)a.y << 32) | a.x);
+    const uint32_t n = b.x;
+    uint32_t bad = 0;
+    switch (a.z) {  // uniform per item
+      case kScanF16: bad = scan_range<kScanF16, 2>(p, n); break;
+      case kScanBF16: bad = scan_range<kScanBF16, 2>(p, n); break;
+      case kScanF32: bad = scan_range<kScanF32, 4>(p, n); break;
+      case kScanF64: bad = scan_range<kScanF64, 8>(p, n); break;
+      case kScanE5M2: bad = scan_range<kScanE5M2, 1>(p, n); break;
+      case kScanE4M3: bad = scan_range<kScanE4M3, 1>(p, n); break;
+      default: break;
+    }
+    bad = __reduce_add_sync(0xffffffffu, bad);
+    if ((threadIdx.x & 31u) == 0 && bad) {
+      add_saturating(counts + b.y, bad);
+      atomicAdd(total, (unsigned long long)bad);
+    }
+  }
+}

@@ -578,6 +578,18 @@ struct fc_plan {
   std::shared_ptr<const DeltaMap> dmap;  // item extents + runs for the incremental drain
   cudaEvent_t ev_upload = nullptr;  // last table upload
   cudaEvent_t ev_last_use = nullptr;  // last kernel that read the tables
+  // non-finite scan: the input ranges as given (empty ones included), one kind byte
+  // each, the scan's own item table (rebuilt on the next scan after a create / update /
+  // kind change) and its result buffers (n uint32 counts + a uint64 total)
+  std::vector<FcSpan> inputs;  // tptr, len (off unused)
+  std::vector<uint8_t> kinds;
+  FcTable scan;
+  bool scan_stale = true;
+  bool scan_enqueued = false;
+  uint8_t* scan_dev = nullptr;
+  uint8_t* scan_host = nullptr;
+  size_t scan_cap = 0;
+  cudaEvent_t ev_scan = nullptr;  // the last scan's result has reached scan_host
 };
 
 static void image_expect_locked(fc_ctx* c, const fc_plan* p, const uint8_t* host,
@@ -1263,6 +1275,11 @@ static int plan_fill(fc_plan* p, uint32_t n, const void* const* dev_ptrs,
   // sit in adjacent but separate device allocations, and a cudaMemcpy must not
   // straddle allocations (kernels do not care, the copy API does).
   p->spans.swap(spans);
+  if (p->kinds.size() != n) p->kinds.assign(n, (uint8_t)FC_KIND_NONE);
+  p->inputs.resize(n);
+  for (uint32_t i = 0; i < n; ++i)
+    p->inputs[i] = {(uint64_t)(uintptr_t)dev_ptrs[i], 0, nbytes[i]};
+  p->scan_stale = true;
   return FC_OK;
 }
 
@@ -1281,6 +1298,7 @@ extern "C" int fc_plan_create(fc_ctx* c, uint32_t n, const void* const* dev_ptrs
   p->chunk = chunk_bytes;
   cudaError_t e = cudaEventCreateWithFlags(&p->ev_upload, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&p->ev_last_use, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&p->ev_scan, cudaEventDisableTiming);
   if (e != cudaSuccess) {
     fc_plan_destroy(p);
     return fail(FC_ECUDA, "fc_plan_create: %s", cudaGetErrorString(e));
@@ -1359,6 +1377,7 @@ extern "C" int fc_plan_destroy(fc_plan* p) {
   // the whole device) and defer the cudaFree (which would sync everything).
   if (p->ev_last_use) cudaEventSynchronize(p->ev_last_use);
   if (p->ev_upload) cudaEventSynchronize(p->ev_upload);
+  if (p->ev_scan) cudaEventSynchronize(p->ev_scan);
   {
     std::lock_guard<std::mutex> lk(c->mu);
     if (c->base_plan == p) {
@@ -1371,12 +1390,15 @@ extern "C" int fc_plan_destroy(fc_plan* p) {
       c->img_map.reset();
     }
   }
-  for (FcTable* t : {&p->all, &p->bulk, &p->resid, &p->shift}) {
+  for (FcTable* t : {&p->all, &p->bulk, &p->resid, &p->shift, &p->scan}) {
     if (t->dev) c->dead_dev.push_back(t->dev);
     if (t->pinned) c->dead_pinned.push_back(t->pinned);
   }
+  if (p->scan_dev) c->dead_dev.push_back(p->scan_dev);
+  if (p->scan_host) c->dead_pinned.push_back(p->scan_host);
   if (p->ev_upload) cudaEventDestroy(p->ev_upload);
   if (p->ev_last_use) cudaEventDestroy(p->ev_last_use);
+  if (p->ev_scan) cudaEventDestroy(p->ev_scan);
   delete p;
   return FC_OK;
 }
@@ -2421,5 +2443,119 @@ extern "C" int fc_restore_timings(fc_ctx* c, float* fill_ms, float* scatter_ms, 
     FC_CUDA(cudaEventElapsedTime(&t, c->ev_fill_start, c->ev_scatter_end));
     *total_ms = t;
   }
+  return FC_OK;
+}
+
+// ---- non-finite scan --------------------------------------------------------------
+static_assert((int)FC_KIND_F16 == (int)kScanF16 && (int)FC_KIND_BF16 == (int)kScanBF16 &&
+                  (int)FC_KIND_F32 == (int)kScanF32 && (int)FC_KIND_F64 == (int)kScanF64 &&
+                  (int)FC_KIND_E5M2 == (int)kScanE5M2 && (int)FC_KIND_E4M3FN == (int)kScanE4M3,
+              "kind codes of the header and the kernel differ");
+
+static uint32_t kind_bytes(uint8_t kind) {
+  switch (kind) {
+    case FC_KIND_F16: case FC_KIND_BF16: return 2;
+    case FC_KIND_F32: return 4;
+    case FC_KIND_F64: return 8;
+    case FC_KIND_E5M2: case FC_KIND_E4M3FN: return 1;
+    default: return 0;
+  }
+}
+
+extern "C" int fc_plan_set_kinds(fc_plan* p, uint32_t n, const uint8_t* kinds) {
+  if (!p || (n && !kinds)) return fail(FC_EINVAL, "fc_plan_set_kinds: null argument%s%s");
+  if (n != p->inputs.size())
+    return fail(FC_EINVAL, "fc_plan_set_kinds: n differs from the plan's number of ranges%s%s");
+  for (uint32_t i = 0; i < n; ++i)
+    if (kinds[i] > FC_KIND_E4M3FN) return fail(FC_EINVAL, "fc_plan_set_kinds: unknown kind%s%s");
+  if (!std::equal(kinds, kinds + n, p->kinds.begin())) {
+    p->kinds.assign(kinds, kinds + n);
+    p->scan_stale = true;
+  }
+  return FC_OK;
+}
+
+extern "C" int fc_scan_nonfinite_async(fc_plan* p, void* stream) {
+  if (!p) return fail(FC_EINVAL, "fc_scan_nonfinite_async: null plan%s%s");
+  fc_ctx* c = p->ctx;
+  FC_GUARD(c);
+  cudaStream_t s = (cudaStream_t)stream;
+  const uint32_t n = (uint32_t)p->inputs.size();
+  // the previous scan may still read the item table and write the result buffers
+  if (p->scan_enqueued) FC_CUDA(cudaEventSynchronize(p->ev_scan));
+  if (p->scan_stale) {
+    // whole elements only: a range clipped inside an element (a window of the segment
+    // cut at any byte) is widened by rounding its address.  Tensor data is
+    // element-aligned, so the widened range stays inside the tensor.
+    std::vector<FcItem> items;
+    for (uint32_t i = 0; i < n; ++i) {
+      const uint32_t es = kind_bytes(p->kinds[i]);
+      const FcSpan& r = p->inputs[i];
+      if (!es || !r.len) continue;
+      uint64_t a = r.tptr & ~(uint64_t)(es - 1);
+      const uint64_t end = (r.tptr + r.len + es - 1) & ~(uint64_t)(es - 1);
+      while (a < end) {
+        // kDefaultChunk is a multiple of every element size: cuts stay on elements
+        const uint64_t len = std::min<uint64_t>(end - a, kDefaultChunk);
+        FcItem it;
+        it.tptr = a;
+        it.aoff = p->kinds[i];
+        it.nbytes = (uint32_t)len;
+        it.pad0 = i;
+        it.pad1 = 0;
+        items.push_back(it);
+        a += len;
+      }
+    }
+    if (items.size() > 0xFFFFFFF0ull) return fail(FC_EINVAL, "scan: too many work items%s%s");
+    int rc = table_set(c, p->scan, items, s, /*sync=*/false);
+    if (rc) return rc;
+    p->scan_stale = false;
+  }
+  const size_t total_at = ((size_t)n * 4 + 7) & ~(size_t)7;  // counts, then the total
+  const size_t bytes = total_at + 8;
+  if (bytes > p->scan_cap) {
+    uint8_t* nd = nullptr;
+    uint8_t* np = nullptr;
+    cudaError_t e = cudaMalloc(&nd, bytes);
+    if (e == cudaSuccess) e = cudaHostAlloc(&np, bytes, cudaHostAllocDefault);
+    if (e != cudaSuccess) {
+      (void)cudaGetLastError();
+      if (nd) c->dead_dev.push_back(nd);
+      return fail(FC_ENOMEM, "scan buffers: %s", cudaGetErrorString(e));
+    }
+    if (p->scan_dev) c->dead_dev.push_back(p->scan_dev);
+    if (p->scan_host) c->dead_pinned.push_back(p->scan_host);
+    p->scan_dev = nd;
+    p->scan_host = np;
+    p->scan_cap = bytes;
+  }
+  FC_CUDA(cudaMemsetAsync(p->scan_dev, 0, bytes, s));
+  if (p->scan.n) {
+    const uint32_t grid =
+        std::min<uint32_t>(p->scan.n, (uint32_t)c->sm_count * (2048u / kLsuThreads));
+    fc_scan_nonfinite<<<grid, kLsuThreads, 0, s>>>(
+        p->scan.dev, p->scan.n, reinterpret_cast<uint32_t*>(p->scan_dev),
+        reinterpret_cast<unsigned long long*>(p->scan_dev + total_at));
+    FC_CUDA(cudaGetLastError());
+    c->n_kernels += 1;
+  }
+  FC_CUDA(cudaMemcpyAsync(p->scan_host, p->scan_dev, bytes, cudaMemcpyDeviceToHost, s));
+  FC_CUDA(cudaEventRecord(p->ev_scan, s));
+  p->scan_enqueued = true;
+  return FC_OK;
+}
+
+extern "C" int fc_scan_wait(fc_plan* p, uint64_t* total, uint32_t* counts, uint32_t n) {
+  if (!p) return fail(FC_EINVAL, "fc_scan_wait: null plan%s%s");
+  if (!p->scan_enqueued) return fail(FC_EINVAL, "fc_scan_wait: no scan was enqueued%s%s");
+  if (counts && n != p->inputs.size())
+    return fail(FC_EINVAL, "fc_scan_wait: n differs from the plan's number of ranges%s%s");
+  FC_GUARD(p->ctx);
+  FC_CUDA(cudaEventSynchronize(p->ev_scan));
+  const size_t nn = p->inputs.size();
+  const size_t total_at = (nn * 4 + 7) & ~(size_t)7;
+  if (counts) memcpy(counts, p->scan_host, nn * 4);
+  if (total) memcpy(total, p->scan_host + total_at, 8);
   return FC_OK;
 }

@@ -522,8 +522,12 @@ class CheckpointEngine(metaclass=ABCMeta):
         seq = ctl.coop_seq() + 1
         patience = float(self._save_timeout) if blocking else 60.0
 
+        coop = CoopContext(ctl, self._local_rank, local_world, seq - 1,
+                           timeout=float(self._save_timeout), opened=not leader)
+        # my window of the image must be finite: the verdict travels with readiness
+        finite = self._part_finite(state_dict, conf, coop, shards) if ready else True
         if not leader:
-            ctl.slot_arrive(self._local_rank, seq, ready)
+            ctl.slot_arrive(self._local_rank, seq, ready and finite)
             try:
                 go = ctl.wait_coop_open(seq, patience)
             except TimeoutError:
@@ -531,12 +535,10 @@ class CheckpointEngine(metaclass=ABCMeta):
                 logger.warning(f"Rank {self._rank}: the node's saving rank did not start save "
                                f"{conf.step} within {patience:.0f}s; not taking part.")
                 return False
-            if not go or not ready:
-                self.is_skip = True
+            if not go or not ready or not finite:
+                self._skipped(conf.step, None if finite else self._non_finite)
                 return False
             state_dict[DLROVER_CKPT_CONFIG_KEY] = conf
-            coop = CoopContext(ctl, self._local_rank, local_world, seq - 1,
-                               timeout=float(self._save_timeout), opened=True)
             if shards:
                 handler.save_shards_as_full(state_dict, coop,
                                             blocking=not self._async_drain or blocking,
@@ -565,19 +567,28 @@ class CheckpointEngine(metaclass=ABCMeta):
                 return self._SOLO
             node_ready = acquired and followers_ready
             all_ready = node_ready
-            if self._saver_group is not None and dist.get_world_size(self._saver_group) > 1:
+            several = self._saver_group is not None and dist.get_world_size(self._saver_group) > 1
+            if several and self.refuse_non_finite:
+                # several nodes: the leaders settle readiness and finiteness in one all-reduce
+                not_ready, non_finite = all_reduce_flags(
+                    self._saver_group, [0 if node_ready else 1, 0 if finite else 1])
+                all_ready, finite = not_ready == 0, non_finite == 0
+            elif several:
                 # several nodes: their leaders settle it like the reference's saving ranks
                 all_ready = check_all_rank_ready(self._saver_group, node_ready)
-            if not all_ready:
+            if not all_ready or not finite:
+                # a follower's slot carries "ready and finite" as one bit: a non-finite
+                # window of a follower reads here as not ready
                 ctl.next_coop_seq(aborted=True)
-                self.is_skip = True
+                claim.release()
+                self._skipped(conf.step, None if finite else self._non_finite)
+                if not finite:
+                    return False
                 logger.info(f"Rank {self._rank} skips the cooperative save of step {conf.step}: "
                             "not every rank is ready (the agent is persisting, or a drain is "
                             "in flight).")
-                claim.release()
                 return False
             state_dict[DLROVER_CKPT_CONFIG_KEY] = conf
-            coop = CoopContext(ctl, 0, local_world, seq - 1, timeout=float(self._save_timeout))
             # the handler opens save `seq` once the segment has its size and the
             # announcement is out; a failed drain leaves writing_shm set (torn segment)
             # and only gives the lock back
@@ -658,6 +669,23 @@ class CheckpointEngine(metaclass=ABCMeta):
     def incremental(self, value: bool):
         self._shm_handler.incremental = bool(value)
 
+    # Refuse memory saves of a non-finite state (opt-in; also DLROVER_B200_REFUSE_NONFINITE=1):
+    # before anything is written, every saving rank scans its part of the state for NaN /
+    # Inf, and if any rank finds one, every rank skips the save; the last checkpoint in
+    # shared memory (and its HBM image, for rollback_into) stays as it was.  Every saving
+    # rank must use the same setting: it changes the readiness all-reduce.
+    _refuse_non_finite: Optional[bool] = None
+
+    @property
+    def refuse_non_finite(self) -> bool:
+        if self._refuse_non_finite is None:
+            return os.getenv("DLROVER_B200_REFUSE_NONFINITE", "0") == "1"
+        return self._refuse_non_finite
+
+    @refuse_non_finite.setter
+    def refuse_non_finite(self, value: bool):
+        self._refuse_non_finite = bool(value)
+
     def wait_snapshot(self):
         """Call before the first write to tensors handed to the last save."""
         self._shm_handler.wait_snapshot()
@@ -708,9 +736,22 @@ class CheckpointEngine(metaclass=ABCMeta):
         claim = ShardLockClaim(self._shm_lock, acquired)
         logger.info(f"{self._rank}-{self._local_rank} acquired the lock of shared memory: "
                     f"{acquired} for step: {conf.step}.")
-        all_rank_ready = check_all_rank_ready(self._saver_group, acquired)
+        if self.refuse_non_finite:
+            # before anything is touched: every saving rank learns whether any part of the
+            # step is non-finite, in the readiness all-reduce (2 ints: refusal and a skip
+            # for the lock stay apart)
+            finite = self._part_finite(state_dict, conf) if acquired and state_dict else True
+            not_ready, non_finite = all_reduce_flags(
+                self._saver_group, [0 if acquired else 1, 0 if finite else 1])
+            if non_finite:
+                claim.release()
+                self._skipped(conf.step, self._non_finite if not finite else {})
+                return False
+            all_rank_ready = not_ready == 0
+        else:
+            all_rank_ready = check_all_rank_ready(self._saver_group, acquired)
         if not all_rank_ready or not state_dict:
-            self.is_skip = True
+            self._skipped(conf.step, None)
             logger.info(f"Rank {self._rank} skips the save the checkpoint in CPU memory since "
                         "it is saving the latest checkpoint from the CPU memory into the "
                         "storage.")
@@ -738,6 +779,37 @@ class CheckpointEngine(metaclass=ABCMeta):
         self._cached_step = conf.step
         return True
 
+    def _part_finite(self, state_dict, conf: CheckpointConfig, coop: Optional[CoopContext] = None,
+                     shards: bool = False) -> bool:
+        """With refuse_non_finite on: whether this rank's part of the save holds no NaN /
+        Inf (the GPU scan of the ranges the save would read, the host check of its CPU
+        leaves); the offenders go to self._non_finite.  True with the switch off."""
+        self._non_finite = {}
+        if not self.refuse_non_finite:
+            return True
+        # the tree the save will walk, conf included, without touching the caller's dict
+        tree = dict(state_dict)
+        tree[DLROVER_CKPT_CONFIG_KEY] = conf
+        self._non_finite = self._shm_handler.scan_nonfinite(
+            tree, stream=self.snapshot_stream, coop=coop, shards=shards, reuse_for=state_dict)
+        return not self._non_finite
+
+    def _skipped(self, step, non_finite: Optional[Dict[str, int]]):
+        """Bookkeeping of a save that did not start; non_finite (not None): it was refused
+        because some saving rank's part holds NaN / Inf (this rank's offenders, maybe none)."""
+        self.is_skip = True
+        if self.refuse_non_finite:
+            self._shm_handler.take_scanned(None)  # the scan's layout holds the tensors
+        if non_finite is None:
+            return
+        self._shm_handler.last_save_stats = {"refused": True, "non_finite": dict(non_finite)}
+        named = ", ".join(f"{k} ({v})" for k, v in list(non_finite.items())[:8])
+        more = f" and {len(non_finite) - 8} more" if len(non_finite) > 8 else ""
+        logger.warning(f"Rank {self._rank} refuses the memory save of step {step}: the state "
+                       "holds NaN/Inf "
+                       + (f"in {named}{more}" if named else "on another rank")
+                       + "; the last checkpoint in memory is kept.")
+
     def wait_memory_save(self, timeout: Optional[float] = None) -> bool:
         """Block until the drain of the last save has landed in shared memory."""
         return self._shm_handler.wait_pending(timeout)
@@ -753,7 +825,10 @@ class CheckpointEngine(metaclass=ABCMeta):
 
     def last_save_stats(self):
         """{"delta": bool, "drained_bytes": int} of the last finished save when it went
-        through the incremental path (delta False: it was a full save), else None."""
+        through the incremental path (delta False: it was a full save);
+        {"refused": True, "non_finite": {leaf path: count}} when refuse_non_finite refused
+        the last save (this rank's offenders: empty when another rank had them); else
+        None."""
         return self._shm_handler.last_save_stats
 
     # -- memory load ---------------------------------------------------------------------

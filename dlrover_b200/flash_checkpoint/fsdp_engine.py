@@ -692,6 +692,9 @@ class FsdpCheckpointEngine(CheckpointEngine):
         of the same structure reuse this rank's final plan and the global metadata and
         run NO collective besides the readiness all-reduce (which carries one more int:
         "my plan changed")."""
+        if self.refuse_non_finite:
+            raise NotImplementedError("refuse_non_finite does not cover sharded (DCP) saves: "
+                                      "switch it off for FsdpCheckpointEngine")
         if self._local_rank != self.local_shard_id:
             return False
         handler, writer = self._shm_handler, self._shm_writer

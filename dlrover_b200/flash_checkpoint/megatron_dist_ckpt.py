@@ -234,6 +234,9 @@ def save_checkpoint(iteration, model, optimizer, opt_param_scheduler,
     checkpointer = MegatronDistCheckpointer.singleton_instance(
         args.save, storage=get_checkpoint_storage(deletion_strategy), comm_backend=comm_backend,
         use_distributed_optimizer=args.use_distributed_optimizer, save_timeout=save_timeout)
+    if checkpointer.engine.refuse_non_finite:
+        raise NotImplementedError("refuse_non_finite does not cover megatron_dist_ckpt saves: "
+                                  "switch it off for this checkpointer")
     model = m.unwrap_model(model)
     m.print_rank_0("saving checkpoint at iteration {:7d} to {}".format(iteration, args.save))
     rng_state = m.get_rng_state()  # collective across DP ranks

@@ -26,6 +26,7 @@ fallback for CUDA leaves: a missing library raises.
 from __future__ import annotations
 
 import atexit
+import bisect
 import copy
 import json
 import os
@@ -457,6 +458,35 @@ def _row_ranges(t: torch.Tensor, off: int, max_rows: int = 1 << 16, min_row_byte
             if idx[d] < sizes[d]:
                 break
             idx[d] = 0
+    return out
+
+
+# kind of the non-finite scan per dtype: complex as its float components; integers, bool
+# and the other float8 kinds are not scanned
+_SCAN_KINDS = {
+    torch.float16: native.KIND_F16, torch.bfloat16: native.KIND_BF16,
+    torch.float32: native.KIND_F32, torch.float64: native.KIND_F64,
+    torch.complex64: native.KIND_F32, torch.complex128: native.KIND_F64,
+    torch.float8_e5m2: native.KIND_E5M2, torch.float8_e4m3fn: native.KIND_E4M3FN,
+}
+
+
+def _leaf_paths(state_dict) -> List[str]:
+    """Dotted path of every tensor leaf (sharded ones included), in the order of the
+    layout walks above."""
+    out: List[str] = []
+
+    def walk(value, path):
+        if isinstance(value, torch.Tensor) or hasattr(value, "local_shards"):
+            out.append(path)
+        elif isinstance(value, Mapping):
+            for k, v in value.items():
+                walk(v, f"{path}.{k}" if path else str(k))
+        elif isinstance(value, list):
+            for i, v in enumerate(value):
+                walk(v, f"{path}.{i}" if path else str(i))
+
+    walk(state_dict, "")
     return out
 
 
@@ -911,6 +941,7 @@ class SharedMemoryHandler:
         self.last_restore_stats: Dict[str, float] = {}
         self.last_hybrid_cut = None
         self._snapshot_ceiling = 0  # largest snapshot arena HBM turned out to have room for
+        self._scanned = None  # (state dict, layout, mine) of the last scan_nonfinite
         self._last_ticket = None
         if not host:
             # a drain still in flight when the interpreter exits must finish (the
@@ -1120,31 +1151,13 @@ class SharedMemoryHandler:
                 native.host_pack(self.shared_memory.address, ptrs, offs, lens, _host_threads())
             del keep
         ctx, ticket = None, 0
-        stager = None
-        prepared = None
         delta = False
-        if device_ranges:
-            stager = self._stager_for([r[0] for r in device_ranges])
-            # a dense repack of an oddly strided leaf runs on the CURRENT stream: do it
-            # before a side stream is made to wait for that stream
-            prepared = stager.prepare_ranges(device_ranges, keepalive)
-            if window is not None:
-                prepared = _clip_ranges(prepared, window[0], window[1])
-                if not prepared[0]:
-                    prepared = None
-        if prepared is not None:
+        got = self._save_plan(device_ranges, keepalive, stream, window, compact)
+        if got is not None:
+            stager, prepared, plan, stream = got
             lo, hi = window if window is not None else (0, self.shared_memory.size)
             stager.attach(self.shared_memory, lo, hi)
             host_addr = self.shared_memory.dma_address + lo
-            current = torch.cuda.current_stream(stager.device_index)
-            if stream is None:
-                stream = current
-            elif stream != current:
-                # snapshot on a side stream: it must see everything the training
-                # stream has enqueued so far, and the caller must make the training
-                # stream wait for `last_pack_event` before it MUTATES the tensors
-                stream.wait_stream(current)
-            plan = stager.plan_for(prepared, role="save", stream=stream, base=lo, compact=compact)
             in_place = (self.in_place if in_place is None else in_place) and not compact
             cut = None  # hybrid: window offset from which the tensors are snapshotted
             if in_place:
@@ -1224,6 +1237,96 @@ class SharedMemoryHandler:
             return None
         self._completion_worker().put(pending)
         return pending
+
+    def _save_plan(self, device_ranges, keepalive: list, stream, window, compact: bool):
+        """(stager, prepared ranges, plan, stream) a save of these CUDA (tensor, segment
+        offset, nbytes) ranges runs with (the save's and the non-finite scan's one plan),
+        or None when there are no device bytes (in the window).  `stream` (default: the
+        current one) is made to wait for the current stream."""
+        if not device_ranges:
+            return None
+        stager = self._stager_for([r[0] for r in device_ranges])
+        # a dense repack of an oddly strided leaf runs on the CURRENT stream: do it
+        # before a side stream is made to wait for that stream
+        prepared = stager.prepare_ranges(device_ranges, keepalive)
+        if window is not None:
+            prepared = _clip_ranges(prepared, window[0], window[1])
+            if not prepared[0]:
+                return None
+        current = torch.cuda.current_stream(stager.device_index)
+        if stream is None:
+            stream = current
+        elif stream != current:
+            # snapshot on a side stream: it must see everything the training
+            # stream has enqueued so far, and the caller must make the training
+            # stream wait for `last_pack_event` before it MUTATES the tensors
+            stream.wait_stream(current)
+        lo = window[0] if window is not None else 0
+        plan = stager.plan_for(prepared, role="save", stream=stream, base=lo, compact=compact)
+        return stager, prepared, plan, stream
+
+    def scan_nonfinite(self, state_dict, stream=None, coop: Optional[CoopContext] = None,
+                       shards: bool = False, reuse_for=None) -> Dict[str, int]:
+        """{leaf path: NaN/Inf count} of the part of `state_dict` that a save through this
+        handler would write from this process ({} when it is finite).  CUDA leaves: the
+        plan the save will use (built or reused here) is scanned on `stream` after it
+        waited for the current stream; CPU leaves are checked on the host.  coop / shards:
+        as save_state_dict(coop=...) / save_shards_as_full.  Touches neither the segment,
+        the meta nor the arena.  reuse_for: the state dict whose save follows right away
+        takes this walk's layout instead of walking again."""
+        mine = None
+        if shards:
+            lay, mine = plan_layout_full_from_shards(state_dict)
+        else:
+            lay = plan_layout(state_dict, self._layout)
+        self._scanned = (reuse_for, lay, mine)
+        metas = [m for m in lay.leaf_metas if m.numel]
+        starts = [m.offset for m in metas]
+        counts: Dict[int, int] = {}  # index into metas -> count
+
+        def owner(off: int) -> int:
+            return bisect.bisect_right(starts, off) - 1
+
+        host = _triples(lay.host_leaves) + [r for r in (mine or ()) if not r[0].is_cuda]
+        for t, off, _ in host:
+            m = metas[owner(off)]
+            if _SCAN_KINDS.get(m.dtype, native.KIND_NONE) == native.KIND_NONE:
+                continue
+            v = t.detach()
+            if v.dtype != m.dtype:  # a byte view of a clipped leaf
+                v = v.view(m.dtype)
+            bad = int((~torch.isfinite(v.float() if v.element_size() == 1 else v)).sum())
+            if bad:
+                counts[owner(off)] = counts.get(owner(off), 0) + bad
+        dev = _triples(lay.device_leaves)
+        window = coop.window(lay.total) if coop is not None else None
+        if mine is not None:
+            dev = _clip_triples(dev, *window) + [r for r in mine if r[0].is_cuda]
+            window = None
+        got = self._save_plan(dev, [], stream, window, compact=mine is not None)
+        if got is not None:
+            _, (_, offs, _), plan, stream = got
+            owners = [owner(o) for o in offs]
+            plan.set_kinds([_SCAN_KINDS.get(metas[i].dtype, native.KIND_NONE) for i in owners])
+            plan.scan_nonfinite_async(stream)
+            total, per_range = plan.scan_wait(len(owners))
+            if total:
+                for i, c in zip(owners, per_range):
+                    if c:
+                        counts[i] = counts.get(i, 0) + c
+        if not counts:
+            return {}
+        paths = {id(m): p for m, p in zip(lay.leaf_metas, _leaf_paths(state_dict))}
+        return {paths.get(id(metas[i]), f"offset {metas[i].offset}"): c
+                for i, c in sorted(counts.items())}
+
+    def take_scanned(self, state_dict):
+        """(layout, mine) of the scan_nonfinite that ran for `state_dict`, or None; the
+        scan's layout is forgotten either way (take_scanned(None) after a skipped save)."""
+        scanned, self._scanned = self._scanned, None
+        if scanned is not None and scanned[0] is not None and scanned[0] is state_dict:
+            return scanned[1], scanned[2]
+        return None
 
     def _completion_worker(self):
         """One long-lived thread per handler finishes the non-blocking saves in order
@@ -1333,7 +1436,8 @@ class SharedMemoryHandler:
         leader runs the meta protocol, the others report through the control segment.
         """
         self.wait_pending()
-        lay = self._layout = plan_layout(state_dict, self._layout)
+        scanned = self.take_scanned(state_dict)
+        lay = self._layout = scanned[0] if scanned else plan_layout(state_dict, self._layout)
         if coop is not None:
             return self._save_cooperative(state_dict, lay, coop, blocking, stream, on_complete,
                                           on_error)
@@ -1384,7 +1488,7 @@ class SharedMemoryHandler:
         drains its own shards to where they belong in the full tensors (plus its slice of
         the replicated leaves).  All ranks that hold shards must be local to this node."""
         self.wait_pending()
-        lay, mine = plan_layout_full_from_shards(state_dict)
+        lay, mine = self.take_scanned(state_dict) or plan_layout_full_from_shards(state_dict)
         self._layout = None  # not comparable with a plain layout
         return self._save_cooperative(state_dict, lay, coop, blocking, stream, on_complete,
                                       on_error, mine=mine)

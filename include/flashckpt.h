@@ -352,6 +352,41 @@ int fc_restore_from_image_async(fc_plan* plan, const void* host_base, void* stre
  * host_base, FC_ENOIMAGE when not (also while the save that would set it has not drained). */
 int fc_image_covers(const fc_plan* plan, const void* host_base);
 
+/* ---- non-finite scan: refuse to overwrite a good checkpoint --------------- */
+
+/* Element kinds of the scan.  A kind names how the exponent field sits in the bytes:
+ * complex64 / complex128 are scanned as FC_KIND_F32 / FC_KIND_F64 components.
+ * FC_KIND_NONE (integers, bool, the float8 kinds not listed) is not scanned. */
+enum {
+  FC_KIND_NONE = 0,
+  FC_KIND_F16 = 1,
+  FC_KIND_BF16 = 2,
+  FC_KIND_F32 = 3,
+  FC_KIND_F64 = 4,
+  FC_KIND_E5M2 = 5,  /* float8_e5m2                                      */
+  FC_KIND_E4M3FN = 6 /* float8_e4m3fn: no Inf, NaN = 0x7F / 0xFF          */
+};
+/* One kind byte per input range of `plan` (n = the n of its last create / update, empty
+ * ranges included).  The kinds survive an fc_plan_update* with the same n (another n
+ * resets them to FC_KIND_NONE).  The scan's item table is built on the next scan after a
+ * create, an update or a change of kinds, and reused by every scan after that. */
+int fc_plan_set_kinds(fc_plan* plan, uint32_t n, const uint8_t* kinds);
+/* Enqueue on `stream` a read-only scan of the plan's source bytes (the tensors, never the
+ * arena) that counts, per input range, the elements whose exponent field is all ones:
+ * NaN or +-Inf (FC_KIND_E4M3FN: its NaN patterns).  A range that starts or ends inside an
+ * element (a slice of the segment cut at any byte) is widened to whole elements by
+ * rounding its address, so an element cut in two is counted by both halves.  No
+ * device-wide synchronisation; the arena, the incremental baseline and the image record
+ * are untouched, and a save may be in flight.  One scan per plan at a time: a second call
+ * first waits for the previous one.  The reference has no such check: its save copies
+ * whatever the tensors hold (ckpt_saver.py:198-231). */
+int fc_scan_nonfinite_async(fc_plan* plan, void* stream);
+/* Block the calling host thread until the plan's last scan has finished (that scan's
+ * event only), then return the total number of hits and, when counts != NULL, one
+ * saturating uint32 count per input range (n must then be the plan's n).  FC_EINVAL when
+ * no scan was enqueued. */
+int fc_scan_wait(fc_plan* plan, uint64_t* total, uint32_t* counts, uint32_t n);
+
 #ifdef __cplusplus
 }
 #endif
