@@ -23,6 +23,7 @@ FC_ECUDA = -2
 FC_ENOMEM = -3
 FC_EBUSY = -4
 FC_ENOIMAGE = -5
+FC_EIO = -6
 FC_ENOTREADY = 1
 
 VARIANT_AUTO = 0
@@ -128,6 +129,7 @@ _SIGNATURES = {
     "fc_restore_timings": (ctypes.c_int, [_vp, _fp, _fp, _fp]),
     "fc_restore_from_image_async": (ctypes.c_int, [_vp, _vp, _vp]),
     "fc_image_covers": (ctypes.c_int, [_vp, _vp]),
+    "fc_restore_file_async": (ctypes.c_int, [_vp, ctypes.c_int, _vp]),
     "fc_plan_set_kinds": (ctypes.c_int, [_vp, _u32, ctypes.POINTER(ctypes.c_uint8)]),
     "fc_scan_nonfinite_async": (ctypes.c_int, [_vp, _vp]),
     "fc_scan_wait": (ctypes.c_int, [_vp, ctypes.POINTER(_u64), ctypes.POINTER(_u32), _u32]),
@@ -325,6 +327,14 @@ class Plan:
             return False
         _check(rc, "fc_restore_from_image_async")
         return True
+
+    def restore_file_async(self, fd: int, stream=None):
+        """Restore from an open file: the plan's host offsets are file offsets into `fd`.
+        Returns once the bytes are on the device, with the scatter enqueued on `stream`;
+        Context.restore_wait / restore_timings apply.  NativeError with code FC_EIO on a
+        short file or a failed read (no tensor changed)."""
+        _check(load_library().fc_restore_file_async(self.handle, int(fd), _stream_ptr(stream)),
+               "fc_restore_file_async")
 
     def image_covers(self, host_ptr: int) -> bool:
         """Whether restore_from_image_async would find an image covering this plan (no

@@ -44,7 +44,9 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <errno.h>
 #include <sys/mman.h>
+#include <sys/stat.h>
 #include <sys/syscall.h>
 #include <unistd.h>
 
@@ -84,6 +86,7 @@ extern "C" const char* fc_strerror(int code) {
     case FC_ENOMEM: return "out of memory";
     case FC_EBUSY: return "a save/restore is still in flight";
     case FC_ENOIMAGE: return "the arena holds no image of the segment for this plan";
+    case FC_EIO: return "reading the source file failed";
     case FC_ENOTREADY: return "not ready";
     default: return "unknown flashckpt error";
   }
@@ -282,12 +285,48 @@ struct StagePiece {
   uint8_t* dev;
   uint8_t* host;
   uint64_t len;
+  uint64_t foff;  // file offset when the source is a file (StageFile), else unused
 };
 
 static void stage_pieces(std::vector<StagePiece>& out, uint8_t* dev, uint8_t* host, uint64_t len,
                          uint64_t slot) {
   for (uint64_t o = 0; o < len; o += slot)
-    out.push_back({dev + o, host + o, std::min<uint64_t>(slot, len - o)});
+    out.push_back({dev + o, host + o, std::min<uint64_t>(slot, len - o), 0});
+}
+
+// A file as the source of a staged fill (fc_restore_file_async): the workers pread each
+// piece's file bytes into their slot instead of a memcpy from a host mapping.  The first
+// short read or I/O error stops every worker and is remembered here.
+struct StageFile {
+  int fd = -1;
+  std::atomic<bool> failed{false};
+  std::mutex mu;
+  uint64_t bad_off = 0;  // file offset of the first byte that could not be read
+  int err_no = 0;        // 0: end of file (short read)
+  bool read(uint8_t* dst, uint64_t len, uint64_t off) {
+    for (uint64_t got = 0; got < len;) {
+      const ssize_t r = pread(fd, dst + got, len - got, (off_t)(off + got));
+      if (r > 0) {
+        got += (uint64_t)r;
+        continue;
+      }
+      if (r < 0 && errno == EINTR) continue;
+      std::lock_guard<std::mutex> lk(mu);
+      if (!failed.load()) {
+        bad_off = off + got;
+        err_no = r < 0 ? errno : 0;
+        failed.store(true);
+      }
+      return false;
+    }
+    return true;
+  }
+};
+
+static void stage_file_pieces(std::vector<StagePiece>& out, uint8_t* dev, uint64_t foff,
+                              uint64_t len, uint64_t slot) {
+  for (uint64_t o = 0; o < len; o += slot)
+    out.push_back({dev + o, nullptr, std::min<uint64_t>(slot, len - o), foff + o});
 }
 
 static cudaError_t stage_worker_init(fc_ctx* c, fc_ctx::StageWorker& w) {
@@ -301,10 +340,11 @@ static cudaError_t stage_worker_init(fc_ctx* c, fc_ctx::StageWorker& w) {
   return e;
 }
 
-// to_host=false: host -> slot (memcpy) -> device (DMA).  true: the inverse.
+// to_host=false: host -> slot (memcpy, or pread from `file`) -> device (DMA).  true: the
+// inverse.
 static void stage_worker(fc_ctx* c, int wi, const std::vector<StagePiece>* pieces,
                          std::atomic<size_t>* next, bool to_host, cudaEvent_t gate,
-                         std::atomic<int>* err) {
+                         std::atomic<int>* err, StageFile* file) {
   cudaSetDevice(c->device);
   fc_ctx::StageWorker& w = c->stage[wi];
   cudaError_t e = stage_worker_init(c, w);
@@ -319,7 +359,11 @@ static void stage_worker(fc_ctx* c, int wi, const std::vector<StagePiece>* piece
       const int sl = j & 1;
       if (used[sl]) e = cudaEventSynchronize(w.ev[sl]);  // the DMA out of this slot is done
       if (e != cudaSuccess) break;
-      memcpy(w.slot[sl], pc.host, pc.len);
+      if (file) {
+        if (file->failed.load() || !file->read(w.slot[sl], pc.len, pc.foff)) break;
+      } else {
+        memcpy(w.slot[sl], pc.host, pc.len);
+      }
       e = cudaMemcpyAsync(pc.dev, w.slot[sl], pc.len, cudaMemcpyHostToDevice, w.stream);
       if (e == cudaSuccess) e = cudaEventRecord(w.ev[sl], w.stream);
       used[sl] = true;
@@ -357,9 +401,10 @@ static void stage_worker(fc_ctx* c, int wi, const std::vector<StagePiece>* piece
   }
 }
 
-// Runs the pieces over `threads` workers (the caller is one of them); blocks.
+// Runs the pieces over `threads` workers (the caller is one of them); blocks.  With a
+// `file`, the caller checks file->failed as well: an I/O error is no CUDA error.
 static cudaError_t stage_run(fc_ctx* c, const std::vector<StagePiece>& pieces, bool to_host,
-                             cudaEvent_t gate, int threads) {
+                             cudaEvent_t gate, int threads, StageFile* file = nullptr) {
   if (pieces.empty()) return cudaSuccess;
   int nt = std::max(1, std::min(threads, 32));
   nt = (int)std::min<size_t>((size_t)nt, pieces.size());
@@ -368,8 +413,8 @@ static cudaError_t stage_run(fc_ctx* c, const std::vector<StagePiece>& pieces, b
   std::atomic<int> err{0};
   std::vector<std::thread> th;
   for (int i = 1; i < nt; ++i)
-    th.emplace_back(stage_worker, c, i, &pieces, &next, to_host, gate, &err);
-  stage_worker(c, 0, &pieces, &next, to_host, gate, &err);
+    th.emplace_back(stage_worker, c, i, &pieces, &next, to_host, gate, &err, file);
+  stage_worker(c, 0, &pieces, &next, to_host, gate, &err, file);
   for (auto& t : th) t.join();
   return (cudaError_t)err.load();
 }
@@ -1632,7 +1677,11 @@ static int save_windowed(fc_plan* p, uint8_t* host, cudaStream_t cs) {
   return FC_OK;
 }
 
-static int restore_windowed(fc_plan* p, const uint8_t* host, cudaStream_t s) {
+// fill(lo, hi, abase) brings the plan's bytes of arena range [lo, hi) into the arena, whose
+// byte 0 stands for offset abase, and returns once they are there (or are queued on the
+// copy stream).
+template <class Fill>
+static int restore_windowed(fc_plan* p, cudaStream_t s, Fill fill) {
   fc_ctx* c = p->ctx;
   std::vector<Window> wins = make_windows(p, c->arena_bytes);
   if (wins.empty() && !p->h_all.empty())
@@ -1640,7 +1689,7 @@ static int restore_windowed(fc_plan* p, const uint8_t* host, cudaStream_t s) {
   FC_CUDA(cudaStreamWaitEvent(s, p->ev_upload, 0));
   FC_CUDA(cudaEventRecord(c->ev_fill_start, c->copy_stream));
   for (const Window& w : wins) {
-    int rc = copy_window<false>(c, p, const_cast<uint8_t*>(host), w.base, w.end, w.abase);
+    int rc = fill(w.base, w.end, w.abase);
     if (rc) return rc;
     FC_CUDA(cudaEventRecord(c->ev_fill_end, c->copy_stream));
     FC_CUDA(cudaStreamWaitEvent(s, c->ev_fill_end, 0));
@@ -2280,7 +2329,10 @@ extern "C" int fc_restore_async(fc_plan* p, const void* host_base, void* stream)
   if (p->arena_end > c->arena_bytes) {
     if (c->arena_bytes < (8ull << 20) || !p->identity)
       return fail(FC_EINVAL, "arena smaller than the plan: call fc_arena_reserve first%s%s");
-    rc = restore_windowed(p, static_cast<const uint8_t*>(host_base), (cudaStream_t)stream);
+    uint8_t* host = const_cast<uint8_t*>(static_cast<const uint8_t*>(host_base));
+    rc = restore_windowed(p, (cudaStream_t)stream, [&](uint64_t lo, uint64_t hi, uint64_t ab) {
+      return copy_window<false>(c, p, host, lo, hi, ab);
+    });
     if (rc) return rc;
     c->restore_inflight = true;
     return FC_OK;
@@ -2313,6 +2365,71 @@ extern "C" int fc_restore_async(fc_plan* p, const void* host_base, void* stream)
                               c->copy_stream));
       c->n_memcpys += 1;
     }
+  FC_CUDA(cudaEventRecord(c->ev_fill_end, c->copy_stream));
+  FC_CUDA(cudaStreamWaitEvent(s, c->ev_fill_end, 0));
+  rc = launch_copy<1>(p, s, FC_VARIANT_AUTO);
+  if (rc) return rc;
+  FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
+  c->restore_inflight = true;
+  return FC_OK;
+}
+
+// ---- restore from a file ------------------------------------------------------------
+// The plan's host offsets are file offsets.  The stage workers pread every run into their
+// pinned bounce slots and DMA each slot into the arena; the scatter is enqueued only once
+// every byte has arrived, so a short read or an I/O error changes no target tensor (in
+// the windowed mode: none after the first window, whose scatter has already run).
+extern "C" int fc_restore_file_async(fc_plan* p, int fd, void* stream) {
+  if (!p || fd < 0) return fail(FC_EINVAL, "fc_restore_file_async: null plan or bad fd%s%s");
+  fc_ctx* c = p->ctx;
+  FC_GUARD(c);
+  int rc = refresh_inflight(c);
+  if (rc) return rc;
+  if (c->save_inflight || c->restore_inflight)
+    return fail(FC_EBUSY, "fc_restore_file_async: arena busy%s%s");
+  delta_forget(c);
+  struct stat st;
+  if (fstat(fd, &st) != 0) return fail(FC_EIO, "fc_restore_file_async: fstat: %s%s", strerror(errno));
+  char at[64], end[64];
+  if (!p->runs.empty() && (uint64_t)st.st_size < p->host_hi) {
+    // a truncated file: refuse before any byte moves, in every mode
+    snprintf(at, sizeof(at), "%llu", (unsigned long long)p->host_hi);
+    snprintf(end, sizeof(end), "%llu", (unsigned long long)st.st_size);
+    return fail(FC_EIO, "fc_restore_file_async: the plan reads up to file offset %s, the file ends at %s",
+                at, end);
+  }
+  StageFile file;
+  file.fd = fd;
+  // the runs' bytes inside arena range [lo, hi) (arena byte 0 = offset ab), read from the file
+  auto fill = [&](uint64_t lo, uint64_t hi, uint64_t ab) -> int {
+    std::vector<StagePiece> pieces;
+    for (const FcRun& r : p->runs) {
+      const uint64_t a = std::max(lo, r.off), b = std::min(hi, r.off + r.len);
+      if (a < b)
+        stage_file_pieces(pieces, c->arena + (a - ab), r.hoff + (a - r.off), b - a, c->stage_slot);
+    }
+    cudaError_t e = stage_run(c, pieces, false, nullptr, c->stage_threads, &file);
+    if (file.failed.load()) {
+      snprintf(at, sizeof(at), "%llu", (unsigned long long)file.bad_off);
+      return fail(FC_EIO, "fc_restore_file_async: read failed at file offset %s: %s", at,
+                  file.err_no ? strerror(file.err_no) : "unexpected end of file");
+    }
+    if (e != cudaSuccess) return fail(FC_ECUDA, "file restore: %s", cudaGetErrorString(e));
+    c->n_memcpys += pieces.size();
+    return FC_OK;
+  };
+  cudaStream_t s = (cudaStream_t)stream;
+  if (p->arena_end > c->arena_bytes) {
+    if (c->arena_bytes < (8ull << 20))
+      return fail(FC_EINVAL, "arena smaller than the plan: call fc_arena_reserve first%s%s");
+    rc = restore_windowed(p, s, fill);
+    if (rc) return rc;
+    c->restore_inflight = true;
+    return FC_OK;
+  }
+  FC_CUDA(cudaEventRecord(c->ev_fill_start, c->copy_stream));
+  rc = fill(0, p->arena_end, 0);  // blocks until the bytes are in the arena
+  if (rc) return rc;
   FC_CUDA(cudaEventRecord(c->ev_fill_end, c->copy_stream));
   FC_CUDA(cudaStreamWaitEvent(s, c->ev_fill_end, 0));
   rc = launch_copy<1>(p, s, FC_VARIANT_AUTO);

@@ -106,7 +106,8 @@ class DdpCheckpointer(Checkpointer):
     def load_checkpoint_into(self, state_dict, stream=None, strict=True):
         """Scatter the in-memory checkpoint into the live tensors of
         `state_dict` (e.g. model.state_dict()); returns the restored step, 0 if
-        memory holds nothing usable (then fall back to load_checkpoint())."""
+        memory holds nothing usable (then fall back to load_storage_into() or
+        load_checkpoint())."""
         step, _ = self._engine.load_into({CheckpointConstant.MODEL_STATES_NAME: state_dict},
                                          stream=stream, strict=strict)
         return step
@@ -119,6 +120,16 @@ class DdpCheckpointer(Checkpointer):
         usable."""
         step, _ = self._engine.rollback_into({CheckpointConstant.MODEL_STATES_NAME: state_dict},
                                              stream=stream, strict=strict)
+        return step
+
+    def load_storage_into(self, state_dict, resume_path="", stream=None, strict=True):
+        """Restore the persisted checkpoint (`resume_path`, else the latest tracked step)
+        straight into the live tensors of `state_dict`, without torch.load: for a node
+        whose shared memory lost the checkpoint (load_checkpoint_into returned 0).
+        Returns the restored step, 0 if nothing is tracked."""
+        step, _ = self._engine.load_storage_into(
+            {CheckpointConstant.MODEL_STATES_NAME: state_dict}, resume_path=resume_path,
+            stream=stream, strict=strict)
         return step
 
     def wait_memory_save(self, timeout=None):

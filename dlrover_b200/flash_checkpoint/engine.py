@@ -23,6 +23,8 @@ Behavioural differences, all on the device path:
   * load_into(): scatter the in-memory checkpoint straight into live tensors.
   * rollback_into(): the same from the HBM snapshot of this process's last save
     when every rank still holds one (no PCIe transfer).
+  * FullCheckpointEngine.load_storage_into(): restore the persisted file straight
+    into live tensors (no torch.load), for a node that lost its memory checkpoint.
 """
 
 from __future__ import annotations
@@ -40,7 +42,7 @@ import torch
 import torch.distributed as dist
 
 from ..common.ctl_segment import ControlSegment
-from ..shm_handler import CoopContext
+from ..shm_handler import CoopContext, restore_file_into
 from ..ckpt_saver import (
     DLROVER_CKPT_CONFIG_KEY,
     AsyncCheckpointSaver,
@@ -1079,6 +1081,37 @@ class FullCheckpointEngine(CheckpointEngine):
         path = self._gen_restore_checkpoint_path(int(content.strip()))
         logger.info(f"Load the state dict from {path}")
         return self.storage.read_state_dict(path, read_func=read)
+
+    def load_storage_into(self, target_state_dict, resume_path="", stream=None, strict=True):
+        """Restore the persisted checkpoint straight into the live tensors of
+        `target_state_dict` ({state name: state dict}, as for load_into), without
+        torch.load: the file is indexed without reading its payload, its bytes are pread
+        through pinned bounce slots into the arena and scattered by the unpack kernels
+        (shm_handler.restore_file_into).  For a node that lost its memory checkpoint.
+        The file is picked as load() picks it: `resume_path`, else the tracked step's
+        file.  Returns (step, stats); (0, {}) when nothing is tracked or the ranks
+        disagree on the step.  With `resume_path` the step is the name of the file's
+        directory (`<dir>/<step>/rank_<r>.pt`), -1 when that is not a number."""
+        names = list(target_state_dict.keys())
+        if len(names) != 1:
+            raise ValueError("The checkpoint file holds the state dict of one path. "
+                             f"Now, paths are {names}")
+        if resume_path:
+            path = resume_path
+            parent = os.path.basename(os.path.dirname(os.path.abspath(path)))
+            step = int(parent) if parent.isdigit() else -1
+        else:
+            tracker = os.path.join(self.checkpoint_dir, CheckpointConstant.TRACER_FILE_NAME)
+            content: str = self.storage.read(tracker)
+            step = int(content.strip()) if content and content.strip() else 0
+            path = self._gen_restore_checkpoint_path(step) if step > 0 else ""
+            passed = verify_all_rank_step_consistent(self._loader_group, step)
+            if not passed or step <= 0:
+                return 0, {}
+        logger.info(f"Restore the state dict from {path} into the live tensors.")
+        stats = restore_file_into(path, target_state_dict[names[0]], stream=stream,
+                                  strict=strict)
+        return step, stats
 
     def _gen_restore_checkpoint_path(self, iteration):
         # unsharded: everyone reads what rank 0 wrote

@@ -1826,3 +1826,254 @@ class SharedMemoryHandler:
 
     def set_master_client(self, client):
         self._master_client = client
+
+
+# -- restore from a torch.save file ----------------------------------------------------
+def _view_rows(shape, stride, first: int, es: int, max_rows: int = 1 << 16):
+    """The bytes of a strided view in logical (row-major) order, as (offset, nbytes) rows
+    starting from element `first`: one row for a dense view, one per dense row when the
+    trailing dims are dense ("row-strided"); None for any other view."""
+    sizes, strides = list(shape), list(stride)
+    k, expect = len(sizes), 1
+    while k > 0 and (sizes[k - 1] == 1 or strides[k - 1] == expect):
+        expect *= sizes[k - 1]
+        k -= 1
+    if k == 0:
+        return [(first * es, expect * es)]
+    n_rows = 1
+    for d in range(k):
+        n_rows *= sizes[d]
+    if (expect == 1 and sizes[-1] != 1) or n_rows > max_rows or any(s < 0 for s in strides[:k]):
+        return None
+    out, idx = [], [0] * k
+    for _ in range(n_rows):
+        out.append(((first + sum(i * s for i, s in zip(idx, strides))) * es, expect * es))
+        for d in range(k - 1, -1, -1):
+            idx[d] += 1
+            if idx[d] < sizes[d]:
+                break
+            idx[d] = 0
+    return out
+
+
+def _pair_rows(src, dst):
+    """Zip the source rows (file offset, n) with the target rows (address, n), both in
+    logical order and of the same total: (address, file offset, n) pieces."""
+    out, i, j, si, dj = [], 0, 0, 0, 0
+    while i < len(src) and j < len(dst):
+        (f, fn), (p, pn) = src[i], dst[j]
+        n = min(fn - si, pn - dj)
+        out.append((p + dj, f + si, n))
+        si, dj = si + n, dj + n
+        if si == fn:
+            i, si = i + 1, 0
+        if dj == pn:
+            j, dj = j + 1, 0
+    return out
+
+
+def _file_targets(index, target, strict: bool):
+    """Pair every tensor leaf of `target` with its TensorLeaf in the file: the tree rules
+    of restore_into (key strictness, exact shape and dtype, non-tensor leaves ignored).
+    Returns [(path, target tensor, leaf)] without 0-element leaves."""
+    from .torch_file_index import TensorLeaf
+
+    pairs = []
+
+    def walk(tgt, src, path):
+        if isinstance(src, Mapping):
+            if not isinstance(tgt, Mapping):
+                raise KeyError(f"{path}: checkpoint has a dict, target has {type(tgt).__name__}")
+            for k, s in src.items():
+                if k not in tgt:
+                    if strict:
+                        raise KeyError(f"{path}{k}: missing in target")
+                    continue
+                walk(tgt[k], s, f"{path}{k}.")
+            if strict:
+                extra = [k for k in tgt if k not in src]
+                if extra:
+                    raise KeyError(f"{path}: target keys not in checkpoint: {extra}")
+        elif isinstance(src, (list, tuple)):
+            if not isinstance(tgt, (list, tuple)) or len(tgt) != len(src):
+                raise KeyError(f"{path}: list length/type mismatch")
+            for i, s in enumerate(src):
+                walk(tgt[i], s, f"{path}{i}.")
+        elif isinstance(src, TensorLeaf):
+            name = path[:-1]
+            if not torch.is_tensor(tgt):
+                raise KeyError(f"{name}: checkpoint has a tensor, target has {type(tgt).__name__}")
+            if tuple(tgt.shape) != src.shape or tgt.dtype != src.dtype:
+                raise ValueError(f"{name}: shape/dtype mismatch {tuple(tgt.shape)}/{tgt.dtype} "
+                                 f"vs {src.shape}/{src.dtype}")
+            if src.numel:
+                pairs.append((name, tgt, src))
+
+    walk(target, index.tree, "")
+    return pairs
+
+
+def _file_ranges(index, pairs):
+    """(target address, file offset, nbytes, leaf path) of every leaf of `pairs`, sorted by
+    file offset.  A range that repeats bytes of another one into the same place (tied
+    weights: two leaves, one storage in the file and one in the model) is dropped."""
+    ranges = []
+    for name, t, leaf in pairs:
+        es = t.element_size()
+        src = _view_rows(leaf.shape, leaf.stride, leaf.storage_offset, es)
+        if src is None:
+            raise ValueError(f"{name}: the file holds a view that is neither dense nor "
+                             f"row-strided (shape {leaf.shape}, stride {leaf.stride}) in "
+                             f"{index.path}")
+        src = [(leaf.file_offset + o, n) for o, n in src]
+        if t.is_contiguous():
+            dst = [(t.data_ptr(), t.numel() * es)]
+        else:
+            rows = _row_ranges(t, 0)
+            if rows is None:
+                raise ValueError(f"{name}: restore needs dense or row-strided CUDA targets "
+                                 f"(got shape {tuple(t.shape)}, strides {t.stride()})")
+            dst = [(p, n) for p, _, n in rows]
+        ranges += [(p, f, n, name) for p, f, n in _pair_rows(src, dst)]
+    ranges.sort(key=lambda r: (r[1], -r[2]))
+    out, live = [], []  # live: kept ranges that reach past the current file offset
+    for r in ranges:
+        live = [k for k in live if k[1] + k[2] > r[1]]
+        if any(r[1] + r[2] <= f + n and r[0] - p == r[1] - f for p, f, n, _ in live):
+            continue
+        out.append(r)
+        live.append(r)
+    return out
+
+
+def _disjoint_groups(ranges):
+    """Split ranges sorted by file offset into groups without overlapping file bytes (a
+    mapped plan reads every file byte once): one group, unless two different tensors are
+    restored from the same bytes (overlapping views of one storage, untied targets)."""
+    groups = []
+    for r in ranges:
+        for g in groups:
+            if g[-1][1] + g[-1][2] <= r[1]:
+                g.append(r)
+                break
+        else:
+            groups.append([r])
+    return groups
+
+
+def _file_arena(ctx: native.Context, plan: native.Plan):
+    """Room for the plan in the arena; when HBM has none, a small arena through which the
+    library streams the plan window by window."""
+    end = plan.arena_end
+    if end <= ctx.arena_info()[1]:
+        return
+    forced = int(os.getenv("DLROVER_B200_ARENA_LIMIT_MB", "0") or 0)
+    if forced:
+        limit = max(8, forced) << 20
+        ctx.set_arena_limit(limit)
+        ctx.arena_reserve(min(end, limit))
+        return
+    try:
+        ctx.arena_reserve(end)
+    except native.NativeError as e:
+        if e.code != native.FC_ENOMEM:
+            raise
+        logger.warning(f"No room for a {end / 2**30:.1f} GiB restore arena in HBM: the file "
+                       "is restored window by window.")
+        ctx.arena_reserve(64 << 20)
+
+
+def _pread_into(fd: int, address: int, nbytes: int, offset: int):
+    import ctypes
+
+    view = memoryview((ctypes.c_char * nbytes).from_address(address)).cast("B")
+    got = 0
+    while got < nbytes:
+        n = os.preadv(fd, [view[got:]], offset + got)
+        if n <= 0:
+            raise OSError(f"short read at file offset {offset + got}")
+        got += n
+
+
+def restore_file_into(path: str, target, stream=None, strict: bool = True,
+                      index=None) -> Dict[str, float]:
+    """Restore the torch.save file at `path` straight into the live tensors of `target`
+    (the tree that was saved: same keys, exact shapes and dtypes, no casts).  The file is
+    indexed without reading its payload (`torch_file_index.index_file`, torch's
+    weights_only unpickler; pass `index` to reuse one).  CUDA leaves: the library preads
+    the file through pinned bounce slots into the arena and scatters it with the unpack
+    kernels (fc_restore_file_async); CPU leaves are pread straight into the tensors.
+    Non-tensor leaves of the file are ignored.  On a short file or a failed read nothing
+    is scattered and the call raises.  The incremental-save baseline and the arena image
+    are forgotten, as by every restore.
+
+    Replaces `sd = torch.load(path, map_location="cpu"); model.load_state_dict(sd)`.
+    stats: device_bytes, host_bytes, read_ms, scatter_ms, wall_ms."""
+    from .torch_file_index import index_file
+
+    t0 = time.perf_counter()
+    if index is None:
+        index = index_file(path)
+    pairs = _file_targets(index, target, strict)
+    dev_pairs = [p for p in pairs if p[1].is_cuda]
+    host_pairs = [p for p in pairs if not p[1].is_cuda]
+    stats = {"device_bytes": 0.0, "host_bytes": 0.0, "read_ms": 0.0, "scatter_ms": 0.0,
+             "wall_ms": 0.0}
+    fd = os.open(path, os.O_RDONLY)
+    try:
+        size = os.fstat(fd).st_size
+        # strided CPU targets are read into a dense copy first (one per target tensor:
+        # tied leaves share it), then torch copies the strides
+        staging = {}
+        for _, t, _ in host_pairs:
+            if not t.is_contiguous() and id(t) not in staging:
+                staging[id(t)] = (t, torch.empty(t.shape, dtype=t.dtype))
+        host = _file_ranges(index, [(n, staging[id(t)][1] if id(t) in staging else t, leaf)
+                                    for n, t, leaf in host_pairs])
+        dev_ranges = _file_ranges(index, dev_pairs)
+        end = max((f + n for _, f, n, _ in host + dev_ranges), default=0)
+        if end > size:  # a truncated file: refuse before any tensor changes
+            raise OSError(f"{path}: the leaves need bytes up to file offset {end}, the file "
+                          f"ends at {size}")
+        with torch.no_grad():
+            if dev_pairs:
+                dev = dev_pairs[0][1].device
+                for name, t, _ in dev_pairs:
+                    if t.device != dev:
+                        raise ValueError(f"{name}: all CUDA leaves must live on one device; "
+                                         f"got {dev} and {t.device}")
+                device_index = dev.index if dev.index is not None else torch.cuda.current_device()
+                ctx = native.get_context(device_index)
+                if stream is None:
+                    stream = torch.cuda.current_stream(device_index)
+                for group in _disjoint_groups(dev_ranges):
+                    ptrs, arena, foffs, lens, a = [], [], [], [], 0
+                    for p, f, n, _ in group:
+                        a += (p - a) % 16  # congruent to the target mod 16: the bulk kernel
+                        ptrs.append(p)
+                        arena.append(a)
+                        foffs.append(f)
+                        lens.append(n)
+                        a += n
+                    plan = ctx.plan(ptrs, arena, lens, host_offsets=foffs)
+                    try:
+                        _file_arena(ctx, plan)
+                        plan.restore_file_async(fd, stream)
+                        ctx.restore_wait()
+                        fill, scatter, _ = ctx.restore_timings()
+                    finally:
+                        plan.destroy()
+                    stats["device_bytes"] += float(plan.payload_bytes)
+                    stats["read_ms"] += fill
+                    stats["scatter_ms"] += scatter
+            t1 = time.perf_counter()
+            for p, f, n, _ in host:
+                _pread_into(fd, p, n, f)
+            for t, s in staging.values():
+                t.copy_(s)
+            stats["read_ms"] += (time.perf_counter() - t1) * 1e3
+            stats["host_bytes"] = float(sum(n for _, _, n, _ in host))
+    finally:
+        os.close(fd)
+    stats["wall_ms"] = (time.perf_counter() - t0) * 1e3
+    return stats

@@ -48,6 +48,7 @@ enum {
   FC_ENOMEM = -3,  /* host or device allocation failed                           */
   FC_EBUSY = -4,   /* a save/restore is still in flight on this context          */
   FC_ENOIMAGE = -5, /* the arena holds no image of the segment for this plan     */
+  FC_EIO = -6,     /* reading the source file failed (short read, I/O error)     */
   FC_ENOTREADY = 1 /* poll: work still pending (not an error)                    */
 };
 
@@ -324,6 +325,26 @@ int fc_restore_direct_async(fc_plan* plan, const void* host_base, void* stream);
 int fc_arena_fill(fc_ctx* ctx, const void* host_base, uint64_t lo, uint64_t hi, void* stream);
 int fc_restore_wait(fc_ctx* ctx);
 int fc_restore_timings(fc_ctx* ctx, float* fill_ms, float* scatter_ms, float* total_ms);
+
+/* ---- restore from a file ---------------------------------------------------- */
+
+/* Restore straight from a file (a torch.save archive the agent persisted): `plan` is a
+ * mapped plan (fc_plan_create_mapped) whose host offsets are FILE offsets into `fd`.  The
+ * stage workers (fc_set_stage) pread each run's bytes into their pinned bounce slots and
+ * DMA every slot into the arena; once all bytes are there, the plan's unpack kernels are
+ * enqueued on `stream`, gated by an event.  No mmap of the file, no cudaHostRegister.
+ * The call returns when the data is on the device; fc_restore_wait / fc_restore_timings
+ * apply (fill = read + DMA).  When the arena is smaller than the plan (>= 8 MiB, a state
+ * that does not fit in HBM twice) the plan is streamed through it window by window, as
+ * fc_restore_async does.  Forgets the incremental baseline and the arena image like every
+ * restore; FC_EBUSY while a save/restore is in flight.
+ * FC_EIO when the file ends before the plan's last byte (checked before anything moves) or
+ * a read fails; fc_last_error() names the file offset.  No scatter is enqueued then, so no
+ * target tensor has changed (windowed mode: a read error after the first window leaves the
+ * earlier windows restored).
+ * Replaces torch.load(path, map_location="cpu") + the per-tensor pageable copy_ of
+ * load_state_dict (reference full_ckpt_engine.py _load_from_storage). */
+int fc_restore_file_async(fc_plan* plan, int fd, void* stream);
 
 /* ---- rollback: restore from the arena image ------------------------------- */
 
