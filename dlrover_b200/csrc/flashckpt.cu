@@ -288,10 +288,12 @@ struct StagePiece {
   uint64_t foff;  // file offset when the source is a file (StageFile), else unused
 };
 
+// Cuts a transfer of len bytes into slot-sized pieces.  host == nullptr: the bytes are read
+// from a file at offset foff.
 static void stage_pieces(std::vector<StagePiece>& out, uint8_t* dev, uint8_t* host, uint64_t len,
-                         uint64_t slot) {
+                         uint64_t slot, uint64_t foff = 0) {
   for (uint64_t o = 0; o < len; o += slot)
-    out.push_back({dev + o, host + o, std::min<uint64_t>(slot, len - o), 0});
+    out.push_back({dev + o, host ? host + o : nullptr, std::min<uint64_t>(slot, len - o), foff + o});
 }
 
 // A file as the source of a staged fill (fc_restore_file_async): the workers pread each
@@ -322,12 +324,6 @@ struct StageFile {
     return true;
   }
 };
-
-static void stage_file_pieces(std::vector<StagePiece>& out, uint8_t* dev, uint64_t foff,
-                              uint64_t len, uint64_t slot) {
-  for (uint64_t o = 0; o < len; o += slot)
-    out.push_back({dev + o, nullptr, std::min<uint64_t>(slot, len - o), foff + o});
-}
 
 static cudaError_t stage_worker_init(fc_ctx* c, fc_ctx::StageWorker& w) {
   cudaError_t e = cudaSuccess;
@@ -1623,8 +1619,7 @@ static std::vector<Window> make_windows(const fc_plan* p, uint64_t arena_bytes) 
   return w;
 }
 
-// DMA the parts of the plan's runs that fall into [lo, hi), one piece at a time.
-template <bool TO_HOST>
+// Drain the parts of the plan's runs that fall into [lo, hi), one piece at a time.
 static int copy_window(fc_ctx* c, const fc_plan* p, uint8_t* host, uint64_t lo, uint64_t hi,
                        uint64_t base) {
   const SliceClip clip(c, host + lo);
@@ -1632,12 +1627,8 @@ static int copy_window(fc_ctx* c, const fc_plan* p, uint8_t* host, uint64_t lo, 
     uint64_t a = std::max(lo, r.off), b = std::min(hi, r.off + r.len);
     for (uint64_t o = a, len = 0; o < b; o += len) {
       len = clip(host + o, std::min<uint64_t>(c->drain_piece, b - o));
-      if (TO_HOST)
-        FC_CUDA(cudaMemcpyAsync(host + o, c->arena + (o - base), len, cudaMemcpyDeviceToHost,
-                                c->copy_stream));
-      else
-        FC_CUDA(cudaMemcpyAsync(c->arena + (o - base), host + o, len, cudaMemcpyHostToDevice,
-                                c->copy_stream));
+      FC_CUDA(cudaMemcpyAsync(host + o, c->arena + (o - base), len, cudaMemcpyDeviceToHost,
+                              c->copy_stream));
       c->n_memcpys += 1;
       FC_CUDA(cudaStreamSynchronize(c->copy_stream));  // paced: one piece in flight
     }
@@ -1662,7 +1653,7 @@ static int save_windowed(fc_plan* p, uint8_t* host, cudaStream_t cs) {
       FC_CUDA(cudaEventRecord(c->ev_drain_start, c->copy_stream));
       first = false;
     }
-    rc = copy_window<true>(c, p, host, w.base, w.end, w.abase);
+    rc = copy_window(c, p, host, w.base, w.end, w.abase);
     if (rc) return rc;
     // the next gather overwrites the window: it must wait for this drain
     FC_CUDA(cudaEventRecord(c->ev_drain_end, c->copy_stream));
@@ -1677,11 +1668,103 @@ static int save_windowed(fc_plan* p, uint8_t* host, cudaStream_t cs) {
   return FC_OK;
 }
 
-// fill(lo, hi, abase) brings the plan's bytes of arena range [lo, hi) into the arena, whose
-// byte 0 stands for offset abase, and returns once they are there (or are queued on the
-// copy stream).
-template <class Fill>
-static int restore_windowed(fc_plan* p, cudaStream_t s, Fill fill) {
+// ---- restores ---------------------------------------------------------------------
+// Every restore refuses while the context is busy, moves the checkpoint's bytes from one
+// source into the arena or the tensors (the fill) and, through the arena, enqueues the
+// plan's unpack kernels on the caller's stream.
+
+// FC_EBUSY with the message `busy` while a save or a restore is in flight.  forget: the
+// restore overwrites what the incremental baseline and the arena image describe.
+static int restore_begin(fc_ctx* c, const char* busy, bool forget = true) {
+  int rc = refresh_inflight(c);
+  if (rc) return rc;
+  if (c->save_inflight || c->restore_inflight) return fail(FC_EBUSY, "%s%s", busy);
+  if (forget) delta_forget(c);
+  return FC_OK;
+}
+
+// One part of a fill: len bytes to device address dev from offset src of the source.
+struct FillSeg {
+  uint8_t* dev;
+  uint64_t src;
+  uint64_t len;
+};
+
+// Where a fill reads: the host mapping `host`, or the file `file` (host unused).
+struct FillSource {
+  const uint8_t* host;
+  StageFile* file;
+  const char* what;  // prefix of the error a failed staged copy returns
+};
+
+// Moves every segment's bytes from src.  A file, or a host range that is not page-locked,
+// goes through the bounce slots (the stage workers start once `gate`, if any, has
+// completed) and is on the device on return.  A page-locked range is queued on the copy
+// stream in kDmaPiece pieces cut at slice boundaries.
+static int restore_fill(fc_ctx* c, const std::vector<FillSeg>& segs, const FillSource& src,
+                        cudaEvent_t gate) {
+  if (segs.empty()) return FC_OK;
+  uint64_t lo = ~0ull, hi = 0;
+  for (const FillSeg& g : segs) {
+    lo = std::min(lo, g.src);
+    hi = std::max(hi, g.src + g.len);
+  }
+  uint8_t* host = const_cast<uint8_t*>(src.host);
+  const int staged = src.file ? c->stage_threads : staged_threads_for(c, host + lo, hi - lo);
+  if (staged > 0) {
+    std::vector<StagePiece> pieces;
+    for (const FillSeg& g : segs)
+      stage_pieces(pieces, g.dev, src.file ? nullptr : host + g.src, g.len, c->stage_slot, g.src);
+    cudaError_t e = stage_run(c, pieces, false, gate, staged, src.file);
+    if (src.file && src.file->failed.load()) {
+      char at[64];
+      snprintf(at, sizeof(at), "%llu", (unsigned long long)src.file->bad_off);
+      return fail(FC_EIO, "fc_restore_file_async: read failed at file offset %s: %s", at,
+                  src.file->err_no ? strerror(src.file->err_no) : "unexpected end of file");
+    }
+    if (e != cudaSuccess) return fail(FC_ECUDA, "%s: %s", src.what, cudaGetErrorString(e));
+    c->n_memcpys += pieces.size();
+    return FC_OK;
+  }
+  const SliceClip clip(c, host + lo);
+  for (const FillSeg& g : segs)
+    for (uint64_t o = 0, len = 0; o < g.len; o += len) {
+      len = clip(host + g.src + o, std::min<uint64_t>(kDmaPiece, g.len - o));
+      FC_CUDA(cudaMemcpyAsync(g.dev + o, host + g.src + o, len, cudaMemcpyHostToDevice,
+                              c->copy_stream));
+      c->n_memcpys += 1;
+    }
+  return FC_OK;
+}
+
+// A fill into memory that work queued on `s` may still use (the tensors of an in-place
+// restore, the arena of fc_arena_fill): it starts once `s` has reached this point, and
+// `s` continues once the bytes are in place.
+static int restore_fill_gated(fc_ctx* c, cudaStream_t s, const std::vector<FillSeg>& segs,
+                              const FillSource& src) {
+  FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
+  FC_CUDA(cudaStreamWaitEvent(c->copy_stream, c->ev_scatter_end, 0));
+  FC_CUDA(cudaEventRecord(c->ev_fill_start, c->copy_stream));
+  int rc = restore_fill(c, segs, src, c->ev_scatter_end);
+  if (rc) return rc;
+  FC_CUDA(cudaEventRecord(c->ev_fill_end, c->copy_stream));
+  FC_CUDA(cudaStreamWaitEvent(s, c->ev_fill_end, 0));
+  return FC_OK;
+}
+
+// The plan's runs inside arena range [lo, hi), into an arena whose byte 0 stands for offset ab.
+static std::vector<FillSeg> run_segs(const fc_plan* p, uint64_t lo, uint64_t hi, uint64_t ab) {
+  std::vector<FillSeg> segs;
+  for (const FcRun& r : p->runs) {
+    const uint64_t a = std::max(lo, r.off), b = std::min(hi, r.off + r.len);
+    if (a < b) segs.push_back({p->ctx->arena + (a - ab), r.hoff + (a - r.off), b - a});
+  }
+  return segs;
+}
+
+// A plan larger than the arena: fill and scatter one window after the other; returns once
+// the last window's scatter is enqueued.
+static int restore_windowed(fc_plan* p, cudaStream_t s, const FillSource& src) {
   fc_ctx* c = p->ctx;
   std::vector<Window> wins = make_windows(p, c->arena_bytes);
   if (wins.empty() && !p->h_all.empty())
@@ -1689,7 +1772,7 @@ static int restore_windowed(fc_plan* p, cudaStream_t s, Fill fill) {
   FC_CUDA(cudaStreamWaitEvent(s, p->ev_upload, 0));
   FC_CUDA(cudaEventRecord(c->ev_fill_start, c->copy_stream));
   for (const Window& w : wins) {
-    int rc = fill(w.base, w.end, w.abase);
+    int rc = restore_fill(c, run_segs(p, w.base, w.end, w.abase), src, nullptr);
     if (rc) return rc;
     FC_CUDA(cudaEventRecord(c->ev_fill_end, c->copy_stream));
     FC_CUDA(cudaStreamWaitEvent(s, c->ev_fill_end, 0));
@@ -1701,6 +1784,32 @@ static int restore_windowed(fc_plan* p, cudaStream_t s, Fill fill) {
   FC_CUDA(cudaEventRecord(c->ev_fill_end, c->copy_stream));
   FC_CUDA(cudaEventRecord(p->ev_last_use, s));
   FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
+  return FC_OK;
+}
+
+// A restore through the arena: fill it from src (window by window when the plan is larger
+// than the arena), then scatter on `s`.  src == nullptr: the arena already holds the bytes
+// (rollback); both fill events go on `s`, so fc_restore_timings reports the scatter alone.
+// The next save, restore or fill refuses (FC_EBUSY) until the scatter has read the arena.
+static int restore_arena(fc_plan* p, cudaStream_t s, const FillSource* src) {
+  fc_ctx* c = p->ctx;
+  if (src && p->arena_end > c->arena_bytes) {
+    int rc = restore_windowed(p, s, *src);
+    if (rc) return rc;
+  } else {
+    cudaStream_t fs = src ? c->copy_stream : s;
+    FC_CUDA(cudaEventRecord(c->ev_fill_start, fs));
+    if (src) {
+      int rc = restore_fill(c, run_segs(p, 0, p->arena_end, 0), *src, nullptr);
+      if (rc) return rc;
+    }
+    FC_CUDA(cudaEventRecord(c->ev_fill_end, fs));
+    FC_CUDA(cudaStreamWaitEvent(s, c->ev_fill_end, 0));
+    int rc = launch_copy<1>(p, s, FC_VARIANT_AUTO);
+    if (rc) return rc;
+    FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
+  }
+  c->restore_inflight = true;
   return FC_OK;
 }
 
@@ -2051,44 +2160,14 @@ extern "C" int fc_restore_direct_async(fc_plan* p, const void* host_base, void* 
     return fail(FC_EINVAL, "fc_restore_direct_async: null argument%s%s");
   fc_ctx* c = p->ctx;
   FC_GUARD(c);
-  int rc = refresh_inflight(c);
+  int rc = restore_begin(c, "fc_restore_direct_async: context busy");
   if (rc) return rc;
-  if (c->save_inflight || c->restore_inflight)
-    return fail(FC_EBUSY, "fc_restore_direct_async: context busy%s%s");
-  delta_forget(c);
   cudaStream_t s = (cudaStream_t)stream;
-  const uint8_t* hb = static_cast<const uint8_t*>(host_base);
-  // the targets may still be read by work queued on `stream`
-  FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
-  FC_CUDA(cudaStreamWaitEvent(c->copy_stream, c->ev_scatter_end, 0));
-  FC_CUDA(cudaEventRecord(c->ev_fill_start, c->copy_stream));
-  const int staged =
-      p->spans.empty() ? 0 : staged_threads_for(c, hb + p->host_lo, p->host_hi - p->host_lo);
-  if (staged > 0) {
-    // unregistered segment (a restarted trainer): bounce slots, blocks until the data
-    // is on the device
-    std::vector<StagePiece> pieces;
-    for (const FcSpan& sp : p->spans)
-      stage_pieces(pieces, (uint8_t*)(uintptr_t)sp.tptr, const_cast<uint8_t*>(hb) + sp.off,
-                   sp.len, c->stage_slot);
-    cudaError_t e = stage_run(c, pieces, false, c->ev_scatter_end, staged);
-    if (e != cudaSuccess) return fail(FC_ECUDA, "staged restore: %s", cudaGetErrorString(e));
-    c->n_memcpys += pieces.size();
-    FC_CUDA(cudaEventRecord(c->ev_fill_end, c->copy_stream));
-    FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
-    c->restore_inflight = true;
-    return FC_OK;
-  }
-  const SliceClip clip(c, hb + p->host_lo);
-  for (const FcSpan& sp : p->spans)
-    for (uint64_t o = 0, len = 0; o < sp.len; o += len) {
-      len = clip(hb + sp.off + o, std::min<uint64_t>(kDmaPiece, sp.len - o));
-      FC_CUDA(cudaMemcpyAsync((uint8_t*)(uintptr_t)sp.tptr + o, hb + sp.off + o, len,
-                              cudaMemcpyHostToDevice, c->copy_stream));
-      c->n_memcpys += 1;
-    }
-  FC_CUDA(cudaEventRecord(c->ev_fill_end, c->copy_stream));
-  FC_CUDA(cudaStreamWaitEvent(s, c->ev_fill_end, 0));
+  std::vector<FillSeg> segs;
+  for (const FcSpan& sp : p->spans) segs.push_back({(uint8_t*)(uintptr_t)sp.tptr, sp.off, sp.len});
+  const FillSource src{static_cast<const uint8_t*>(host_base), nullptr, "staged restore"};
+  rc = restore_fill_gated(c, s, segs, src);
+  if (rc) return rc;
   FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
   c->restore_inflight = true;
   return FC_OK;
@@ -2321,57 +2400,12 @@ extern "C" int fc_restore_async(fc_plan* p, const void* host_base, void* stream)
   if (!p || (!host_base && p->payload)) return fail(FC_EINVAL, "fc_restore_async: null argument%s%s");
   fc_ctx* c = p->ctx;
   FC_GUARD(c);
-  int rc = refresh_inflight(c);
+  int rc = restore_begin(c, "fc_restore_async: arena busy");
   if (rc) return rc;
-  if (c->save_inflight || c->restore_inflight)
-    return fail(FC_EBUSY, "fc_restore_async: arena busy%s%s");
-  delta_forget(c);
-  if (p->arena_end > c->arena_bytes) {
-    if (c->arena_bytes < (8ull << 20) || !p->identity)
-      return fail(FC_EINVAL, "arena smaller than the plan: call fc_arena_reserve first%s%s");
-    uint8_t* host = const_cast<uint8_t*>(static_cast<const uint8_t*>(host_base));
-    rc = restore_windowed(p, (cudaStream_t)stream, [&](uint64_t lo, uint64_t hi, uint64_t ab) {
-      return copy_window<false>(c, p, host, lo, hi, ab);
-    });
-    if (rc) return rc;
-    c->restore_inflight = true;
-    return FC_OK;
-  }
-  cudaStream_t s = (cudaStream_t)stream;
-  const uint8_t* hb = static_cast<const uint8_t*>(host_base);
-  FC_CUDA(cudaEventRecord(c->ev_fill_start, c->copy_stream));
-  const int staged =
-      p->runs.empty() ? 0 : staged_threads_for(c, hb + p->host_lo, p->host_hi - p->host_lo);
-  if (staged > 0) {
-    std::vector<StagePiece> pieces;
-    for (const FcRun& r : p->runs)
-      stage_pieces(pieces, c->arena + r.off, const_cast<uint8_t*>(hb) + r.hoff, r.len,
-                   c->stage_slot);
-    cudaError_t e = stage_run(c, pieces, false, nullptr, staged);
-    if (e != cudaSuccess) return fail(FC_ECUDA, "staged restore: %s", cudaGetErrorString(e));
-    c->n_memcpys += pieces.size();
-    FC_CUDA(cudaEventRecord(c->ev_fill_end, c->copy_stream));
-    rc = launch_copy<1>(p, s, FC_VARIANT_AUTO);  // the fill has completed on the host side
-    if (rc) return rc;
-    FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
-    c->restore_inflight = true;
-    return FC_OK;
-  }
-  const SliceClip clip(c, hb + p->host_lo);
-  for (const FcRun& r : p->runs)
-    for (uint64_t o = 0, len = 0; o < r.len; o += len) {
-      len = clip(hb + r.hoff + o, std::min<uint64_t>(kDmaPiece, r.len - o));
-      FC_CUDA(cudaMemcpyAsync(c->arena + r.off + o, hb + r.hoff + o, len, cudaMemcpyHostToDevice,
-                              c->copy_stream));
-      c->n_memcpys += 1;
-    }
-  FC_CUDA(cudaEventRecord(c->ev_fill_end, c->copy_stream));
-  FC_CUDA(cudaStreamWaitEvent(s, c->ev_fill_end, 0));
-  rc = launch_copy<1>(p, s, FC_VARIANT_AUTO);
-  if (rc) return rc;
-  FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
-  c->restore_inflight = true;
-  return FC_OK;
+  if (p->arena_end > c->arena_bytes && (c->arena_bytes < (8ull << 20) || !p->identity))
+    return fail(FC_EINVAL, "arena smaller than the plan: call fc_arena_reserve first%s%s");
+  const FillSource src{static_cast<const uint8_t*>(host_base), nullptr, "staged restore"};
+  return restore_arena(p, (cudaStream_t)stream, &src);
 }
 
 // ---- restore from a file ------------------------------------------------------------
@@ -2383,11 +2417,8 @@ extern "C" int fc_restore_file_async(fc_plan* p, int fd, void* stream) {
   if (!p || fd < 0) return fail(FC_EINVAL, "fc_restore_file_async: null plan or bad fd%s%s");
   fc_ctx* c = p->ctx;
   FC_GUARD(c);
-  int rc = refresh_inflight(c);
+  int rc = restore_begin(c, "fc_restore_file_async: arena busy");
   if (rc) return rc;
-  if (c->save_inflight || c->restore_inflight)
-    return fail(FC_EBUSY, "fc_restore_file_async: arena busy%s%s");
-  delta_forget(c);
   struct stat st;
   if (fstat(fd, &st) != 0) return fail(FC_EIO, "fc_restore_file_async: fstat: %s%s", strerror(errno));
   char at[64], end[64];
@@ -2398,45 +2429,12 @@ extern "C" int fc_restore_file_async(fc_plan* p, int fd, void* stream) {
     return fail(FC_EIO, "fc_restore_file_async: the plan reads up to file offset %s, the file ends at %s",
                 at, end);
   }
+  if (p->arena_end > c->arena_bytes && c->arena_bytes < (8ull << 20))
+    return fail(FC_EINVAL, "arena smaller than the plan: call fc_arena_reserve first%s%s");
   StageFile file;
   file.fd = fd;
-  // the runs' bytes inside arena range [lo, hi) (arena byte 0 = offset ab), read from the file
-  auto fill = [&](uint64_t lo, uint64_t hi, uint64_t ab) -> int {
-    std::vector<StagePiece> pieces;
-    for (const FcRun& r : p->runs) {
-      const uint64_t a = std::max(lo, r.off), b = std::min(hi, r.off + r.len);
-      if (a < b)
-        stage_file_pieces(pieces, c->arena + (a - ab), r.hoff + (a - r.off), b - a, c->stage_slot);
-    }
-    cudaError_t e = stage_run(c, pieces, false, nullptr, c->stage_threads, &file);
-    if (file.failed.load()) {
-      snprintf(at, sizeof(at), "%llu", (unsigned long long)file.bad_off);
-      return fail(FC_EIO, "fc_restore_file_async: read failed at file offset %s: %s", at,
-                  file.err_no ? strerror(file.err_no) : "unexpected end of file");
-    }
-    if (e != cudaSuccess) return fail(FC_ECUDA, "file restore: %s", cudaGetErrorString(e));
-    c->n_memcpys += pieces.size();
-    return FC_OK;
-  };
-  cudaStream_t s = (cudaStream_t)stream;
-  if (p->arena_end > c->arena_bytes) {
-    if (c->arena_bytes < (8ull << 20))
-      return fail(FC_EINVAL, "arena smaller than the plan: call fc_arena_reserve first%s%s");
-    rc = restore_windowed(p, s, fill);
-    if (rc) return rc;
-    c->restore_inflight = true;
-    return FC_OK;
-  }
-  FC_CUDA(cudaEventRecord(c->ev_fill_start, c->copy_stream));
-  rc = fill(0, p->arena_end, 0);  // blocks until the bytes are in the arena
-  if (rc) return rc;
-  FC_CUDA(cudaEventRecord(c->ev_fill_end, c->copy_stream));
-  FC_CUDA(cudaStreamWaitEvent(s, c->ev_fill_end, 0));
-  rc = launch_copy<1>(p, s, FC_VARIANT_AUTO);
-  if (rc) return rc;
-  FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
-  c->restore_inflight = true;
-  return FC_OK;
+  const FillSource src{nullptr, &file, "file restore"};
+  return restore_arena(p, (cudaStream_t)stream, &src);
 }
 
 // ---- rollback from the arena image ----------------------------------------------
@@ -2471,10 +2469,8 @@ extern "C" int fc_restore_from_image_async(fc_plan* p, const void* host_base, vo
     return fail(FC_EINVAL, "fc_restore_from_image_async: null argument%s%s");
   fc_ctx* c = p->ctx;
   FC_GUARD(c);
-  int rc = refresh_inflight(c);
+  int rc = restore_begin(c, "fc_restore_from_image_async: context busy", false);
   if (rc) return rc;
-  if (c->save_inflight || c->restore_inflight)
-    return fail(FC_EBUSY, "fc_restore_from_image_async: context busy%s%s");
   {
     // nothing runs between this check and the scatter's enqueue that could change the
     // record: saves, restores and plan updates of this context refuse while it is busy,
@@ -2483,55 +2479,19 @@ extern "C" int fc_restore_from_image_async(fc_plan* p, const void* host_base, vo
     if (!image_covers_locked(c, p, static_cast<const uint8_t*>(host_base)))
       return fail(FC_ENOIMAGE, "fc_restore_from_image_async: no arena image covers the plan%s%s");
   }
-  cudaStream_t s = (cudaStream_t)stream;
-  // no fill: both fill events on `stream`, so fc_restore_timings reports fill 0 and the
-  // scatter alone
-  FC_CUDA(cudaEventRecord(c->ev_fill_start, s));
-  FC_CUDA(cudaEventRecord(c->ev_fill_end, s));
-  rc = launch_copy<1>(p, s, FC_VARIANT_AUTO);
-  if (rc) return rc;
-  // the next save, restore or fill refuses (FC_EBUSY) until the scatter has read the arena
-  FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
-  c->restore_inflight = true;
-  return FC_OK;
+  return restore_arena(p, (cudaStream_t)stream, nullptr);
 }
 
 extern "C" int fc_arena_fill(fc_ctx* c, const void* host_base, uint64_t lo, uint64_t hi,
                              void* stream) {
   if (!c || !host_base || hi < lo) return fail(FC_EINVAL, "fc_arena_fill: bad argument%s%s");
   FC_GUARD(c);
-  int rc = refresh_inflight(c);
+  int rc = restore_begin(c, "fc_arena_fill: arena busy");
   if (rc) return rc;
-  if (c->save_inflight || c->restore_inflight)
-    return fail(FC_EBUSY, "fc_arena_fill: arena busy%s%s");
-  delta_forget(c);
   if (hi > c->arena_bytes) return fail(FC_EINVAL, "fc_arena_fill: arena too small%s%s");
   if (hi == lo) return FC_OK;
-  cudaStream_t s = (cudaStream_t)stream;
-  const uint8_t* hb = static_cast<const uint8_t*>(host_base);
-  // whatever `stream` still does with the arena must be over first
-  FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
-  FC_CUDA(cudaStreamWaitEvent(c->copy_stream, c->ev_scatter_end, 0));
-  FC_CUDA(cudaEventRecord(c->ev_fill_start, c->copy_stream));
-  const int staged = staged_threads_for(c, hb + lo, hi - lo);
-  if (staged > 0) {
-    std::vector<StagePiece> pieces;
-    stage_pieces(pieces, c->arena + lo, const_cast<uint8_t*>(hb) + lo, hi - lo, c->stage_slot);
-    cudaError_t e = stage_run(c, pieces, false, c->ev_scatter_end, staged);
-    if (e != cudaSuccess) return fail(FC_ECUDA, "fc_arena_fill (staged): %s", cudaGetErrorString(e));
-    c->n_memcpys += pieces.size();
-    FC_CUDA(cudaEventRecord(c->ev_fill_end, c->copy_stream));
-  } else {
-    const SliceClip clip(c, hb + lo);
-    for (uint64_t o = lo, len = 0; o < hi; o += len) {
-      len = clip(hb + o, std::min<uint64_t>(kDmaPiece, hi - o));
-      FC_CUDA(cudaMemcpyAsync(c->arena + o, hb + o, len, cudaMemcpyHostToDevice, c->copy_stream));
-      c->n_memcpys += 1;
-    }
-    FC_CUDA(cudaEventRecord(c->ev_fill_end, c->copy_stream));
-    FC_CUDA(cudaStreamWaitEvent(s, c->ev_fill_end, 0));
-  }
-  return FC_OK;
+  const FillSource src{static_cast<const uint8_t*>(host_base), nullptr, "fc_arena_fill (staged)"};
+  return restore_fill_gated(c, (cudaStream_t)stream, {{c->arena + lo, lo, hi - lo}}, src);
 }
 
 extern "C" int fc_restore_wait(fc_ctx* c) {

@@ -662,37 +662,44 @@ class _DeviceStager:
 
     ARENA_FULL, ARENA_WINDOWED, ARENA_NONE = "full", "windowed", "none"
 
-    def ensure_arena(self, plan) -> str:
-        """Make room for the snapshot of `plan` in HBM.
-        "full": the arena covers the plan (the training stream then only waits for
-        the gather kernel).  "windowed": DLROVER_B200_ARENA_LIMIT_MB caps the arena
-        and the checkpoint is streamed through it window by window (blocking).
-        "none": HBM has no room for a second copy of the state — the caller saves
-        in place instead (DMA straight from the tensors)."""
-        end = plan.arena_end
-        if end <= self.ctx.arena_info()[1]:
-            return self.ARENA_FULL
+    @classmethod
+    def reserve_arena(cls, ctx: native.Context, end: int) -> str:
+        """Make room in the arena of `ctx` for a plan that ends at arena offset `end`.
+        "full": the arena covers the plan.  "windowed": DLROVER_B200_ARENA_LIMIT_MB caps
+        the arena below the plan, which is then streamed through it window by window.
+        "none": HBM has no room for it."""
+        if end <= ctx.arena_info()[1]:
+            return cls.ARENA_FULL
         forced = int(os.getenv("DLROVER_B200_ARENA_LIMIT_MB", "0") or 0)
         if forced:
             limit = max(8, forced) << 20
-            self.ctx.set_arena_limit(limit)
-            self.ctx.arena_reserve(min(end, limit))
-            return self.ARENA_FULL if end <= limit else self.ARENA_WINDOWED
+            ctx.set_arena_limit(limit)
+            ctx.arena_reserve(min(end, limit))
+            return cls.ARENA_FULL if end <= limit else cls.ARENA_WINDOWED
         try:
-            self.ctx.arena_reserve(end)
-            return self.ARENA_FULL
+            ctx.arena_reserve(end)
+            return cls.ARENA_FULL
         except native.NativeError as e:
             if e.code != native.FC_ENOMEM:
                 raise
-        if not self._warned_no_arena:
+        return cls.ARENA_NONE
+
+    def ensure_arena(self, plan) -> str:
+        """Make room for the snapshot of `plan` in HBM (reserve_arena).  "full": the
+        training stream then only waits for the gather kernel.  "windowed": saves and
+        restores block.  "none": the caller saves in place instead (DMA straight from
+        the tensors)."""
+        mode = self.reserve_arena(self.ctx, plan.arena_end)
+        if mode == self.ARENA_NONE and not self._warned_no_arena:
             self._warned_no_arena = True
             free, _ = torch.cuda.mem_get_info(self.device_index)
             logger.warning(
-                f"No room for a {end / 2**30:.1f} GiB snapshot arena in HBM ({free / 2**30:.1f} "
-                "GiB free): checkpoints are drained in place (DMA straight from the tensors). "
-                "Saves block until the data is in shared memory unless the engine runs with "
-                "in_place=True and the optimizer is guarded (see README, 'in-place saves').")
-        return self.ARENA_NONE
+                f"No room for a {plan.arena_end / 2**30:.1f} GiB snapshot arena in HBM "
+                f"({free / 2**30:.1f} GiB free): checkpoints are drained in place (DMA straight "
+                "from the tensors). Saves block until the data is in shared memory unless the "
+                "engine runs with in_place=True and the optimizer is guarded (see README, "
+                "'in-place saves').")
+        return mode
 
     def close(self):
         for p in self._plans.values():
@@ -893,6 +900,65 @@ class _MetaPlane:
 
     def __bool__(self):
         return True
+
+
+# --------------------------------------------------------------------- restores --
+
+
+def _match_tree(target, tree, leaf_type, sequences, strict: bool):
+    """Pair every `leaf_type` leaf of the checkpoint `tree` with the tensor at the same
+    place in `target`: the tree rules of every restore.  Mappings match by key (the meta
+    header key is skipped; a key on one side only raises when strict), `sequences` by
+    position and length; the shape and dtype must be exact; other leaves are ignored.
+    Returns [(path, target tensor, leaf)] without 0-element leaves."""
+    pairs = []
+
+    def walk(tgt, src, path):
+        if isinstance(src, Mapping):
+            if not isinstance(tgt, Mapping):
+                raise KeyError(f"{path}: checkpoint has a dict, target has {type(tgt).__name__}")
+            for k, s in src.items():
+                if k == DLROVER_CKPT_CONFIG_KEY:
+                    continue
+                sub = f"{path}.{k}" if path else str(k)
+                if k not in tgt:
+                    if strict:
+                        raise KeyError(f"{sub}: missing in target")
+                    continue
+                walk(tgt[k], s, sub)
+            if strict:
+                extra = [k for k in tgt if k not in src]
+                if extra:
+                    raise KeyError(f"{path}: target keys not in checkpoint: {extra}")
+        elif isinstance(src, sequences):
+            if not isinstance(tgt, sequences) or len(tgt) != len(src):
+                raise KeyError(f"{path}: list length/type mismatch")
+            for i, s in enumerate(src):
+                walk(tgt[i], s, f"{path}.{i}" if path else str(i))
+        elif isinstance(src, leaf_type):
+            if not torch.is_tensor(tgt):
+                raise KeyError(f"{path}: checkpoint has a tensor, target has {type(tgt).__name__}")
+            if tuple(tgt.shape) != tuple(src.shape) or tgt.dtype != src.dtype:
+                raise ValueError(f"{path}: shape/dtype mismatch {tuple(tgt.shape)}/{tgt.dtype} "
+                                 f"vs {tuple(src.shape)}/{src.dtype}")
+            if src.numel:
+                pairs.append((path, tgt, src))
+
+    walk(target, tree, "")
+    return pairs
+
+
+def _timed_restore(ctx: native.Context, plan, enqueue) -> Optional[Dict[str, float]]:
+    """Run the restore of `plan` that enqueue() starts and wait for it: device_bytes,
+    fill_ms, scatter_ms, wall_ms.  None when enqueue() returns False (nothing started)."""
+    t0 = time.perf_counter()
+    if enqueue() is False:
+        return None
+    ctx.restore_wait()
+    wall_ms = (time.perf_counter() - t0) * 1e3
+    fill, scatter, _ = ctx.restore_timings()
+    return {"device_bytes": float(plan.payload_bytes), "fill_ms": fill, "scatter_ms": scatter,
+            "wall_ms": wall_ms}
 
 
 # --------------------------------------------------------------------- handler --
@@ -1583,7 +1649,8 @@ class SharedMemoryHandler:
         return state_dict
 
     def restore_into(self, target, stream=None, strict: bool = True,
-                     pin_after: bool = True, coop=None) -> Dict[str, float]:
+                     pin_after: bool = True, coop=None, *,
+                     image_first: bool = False) -> Dict[str, float]:
         """Scatter the in-memory checkpoint straight into the live tensors of
         `target` (same tree structure as what was saved; extra keys on either
         side raise when strict).  CUDA leaves: one DMA fill of the arena + one
@@ -1597,17 +1664,26 @@ class SharedMemoryHandler:
         coop=(index, n, process_group): a REPLICATED state that all n local ranks
         restore at the same time — each rank reads only 1/n of the image from host
         memory into its arena and the slices are exchanged over NVLink (NCCL
-        all-gather, in place) before the scatter kernel; every rank must call."""
-        device_pairs, host_pairs = self._restore_targets(target, strict)
+        all-gather, in place) before the scatter kernel; every rank must call.
+
+        image_first: scatter the CUDA leaves from the arena image when it covers them
+        (see rollback_into); stats then carry "from_image" (1.0 / 0.0)."""
+        device_ranges, host_pairs = self._restore_targets(target, strict)
         stats = {"device_bytes": 0.0, "host_bytes": 0.0, "fill_ms": 0.0, "scatter_ms": 0.0}
+        if image_first:
+            stats["from_image"] = 0.0
         with torch.no_grad():
             stats["host_bytes"] = self._restore_host_leaves(host_pairs)
-            if device_pairs:
-                stager, plan, stream = self._restore_plan(device_pairs, stream)
-                if coop is not None:
-                    stats.update(self._run_restore_cooperative(stager, plan, stream, coop))
-                else:
-                    stats.update(self._run_restore(stager, plan, stream, pin_after=pin_after))
+            if device_ranges:
+                stager, plan, stream = self._restore_plan(device_ranges, stream)
+                got = self._run_rollback(stager, plan, stream) if image_first else None
+                if got is None and coop is not None:
+                    got = self._run_restore_cooperative(stager, plan, stream, coop)
+                elif got is None:
+                    got = self._run_restore(stager, plan, stream, pin_after=pin_after)
+                    if image_first:
+                        got["from_image"] = self.last_restore_stats["from_image"] = 0.0
+                stats.update(got)
         return stats
 
     def rollback_into(self, target, stream=None, strict: bool = True) -> Dict[str, float]:
@@ -1619,34 +1695,22 @@ class SharedMemoryHandler:
         hybrid, bounded-arena or cooperative saves, a restore or anything else that
         rewrote the arena since) this is restore_into.  CPU leaves come from the segment
         either way.  stats: those of restore_into plus "from_image" (1.0 / 0.0)."""
-        device_pairs, host_pairs = self._restore_targets(target, strict)
-        stats = {"device_bytes": 0.0, "host_bytes": 0.0, "fill_ms": 0.0, "scatter_ms": 0.0,
-                 "from_image": 0.0}
-        with torch.no_grad():
-            stats["host_bytes"] = self._restore_host_leaves(host_pairs)
-            if device_pairs:
-                stager, plan, stream = self._restore_plan(device_pairs, stream)
-                got = self._run_rollback(stager, plan, stream)
-                if got is None:
-                    got = self._run_restore(stager, plan, stream)
-                    got["from_image"] = self.last_restore_stats["from_image"] = 0.0
-                stats.update(got)
-        return stats
+        return self.restore_into(target, stream, strict, image_first=True)
 
     def can_rollback(self, target, strict: bool = True) -> bool:
         """Whether rollback_into(target) would scatter every CUDA leaf from the arena
         image; restores nothing.  False when the tree has no CUDA leaf."""
-        device_pairs, _ = self._restore_targets(target, strict)
-        if not device_pairs:
+        device_ranges, _ = self._restore_targets(target, strict)
+        if not device_ranges:
             return False
-        _, plan, _ = self._restore_plan(device_pairs, None)
+        _, plan, _ = self._restore_plan(device_ranges, None)
         return plan.image_covers(self.shared_memory.dma_address)
 
     def _restore_targets(self, target, strict: bool):
         """The part every restore of the in-memory checkpoint into live tensors shares:
         wait for this handler's own drain, refuse a checkpoint that is being written, map
-        the segment, and pair each tensor leaf of `target` with its meta (tree, strictness,
-        shape and dtype checks).  Returns (CUDA pairs, CPU pairs)."""
+        the segment, and pair each tensor leaf of `target` with its meta (_match_tree).
+        Returns (CUDA (tensor, segment offset, nbytes) ranges, CPU (tensor, meta) pairs)."""
         self.wait_pending()
         meta_dict = self.metadata.get()
         config = meta_dict.get(DLROVER_CKPT_CONFIG_KEY, CheckpointConfig())
@@ -1655,43 +1719,11 @@ class SharedMemoryHandler:
         self.refresh_mapping()
         if not self.shared_memory:
             raise RuntimeError("the checkpoint segment does not exist")
-
-        device_pairs: List[Tuple[torch.Tensor, TensorMeta]] = []
-        host_pairs: List[Tuple[torch.Tensor, TensorMeta]] = []
-
-        def walk(tgt, meta, path):
-            if isinstance(meta, Mapping):
-                if not isinstance(tgt, Mapping):
-                    raise KeyError(f"{path}: checkpoint has a dict, target has {type(tgt).__name__}")
-                for k, m in meta.items():
-                    if k == DLROVER_CKPT_CONFIG_KEY:
-                        continue
-                    if k not in tgt:
-                        if strict:
-                            raise KeyError(f"{path}{k}: missing in target")
-                        continue
-                    walk(tgt[k], m, f"{path}{k}.")
-                if strict:
-                    extra = [k for k in tgt if k not in meta]
-                    if extra:
-                        raise KeyError(f"{path}: target keys not in checkpoint: {extra}")
-            elif isinstance(meta, list):
-                if not isinstance(tgt, list) or len(tgt) != len(meta):
-                    raise KeyError(f"{path}: list length/type mismatch")
-                for i, m in enumerate(meta):
-                    walk(tgt[i], m, f"{path}{i}.")
-            elif isinstance(meta, TensorMeta):
-                if not torch.is_tensor(tgt):
-                    raise KeyError(f"{path}: checkpoint has a tensor, target has {type(tgt).__name__}")
-                if tuple(tgt.shape) != tuple(meta.shape) or tgt.dtype != meta.dtype:
-                    raise ValueError(
-                        f"{path}: shape/dtype mismatch {tuple(tgt.shape)}/{tgt.dtype} vs "
-                        f"{tuple(meta.shape)}/{meta.dtype}")
-                if meta.numel:
-                    (device_pairs if tgt.is_cuda else host_pairs).append((tgt, meta))
-
-        walk(target, meta_dict, "")
-        return device_pairs, host_pairs
+        # tuples are leaves of the memory checkpoint (plan_layout does not descend into them)
+        pairs = _match_tree(target, meta_dict, TensorMeta, (list,), strict)
+        device_ranges = [(t, m.offset, m.numel * m.element_size) for _, t, m in pairs if t.is_cuda]
+        host_pairs = [(t, m) for _, t, m in pairs if not t.is_cuda]
+        return device_ranges, host_pairs
 
     def _restore_host_leaves(self, host_pairs) -> float:
         """CPU leaves straight from the segment; returns their bytes."""
@@ -1705,13 +1737,11 @@ class SharedMemoryHandler:
                                [m.numel * m.element_size for _, m in dense], _host_threads())
         return float(sum(m.numel * m.element_size for _, m in host_pairs))
 
-    def _restore_plan(self, device_pairs, stream):
-        """(stager, restore plan, stream) for the CUDA leaves: arena offset = segment
-        offset of every leaf, so the plan lines up with the saves' arena image."""
-        stager = self._stager_for([t for t, _ in device_pairs])
-        prepared = stager.prepare_ranges(
-            [(t, m.offset, m.numel * m.element_size) for t, m in device_pairs], [],
-            for_write=True)
+    def _restore_plan(self, device_ranges, stream):
+        """(stager, restore plan, stream) for (CUDA tensor, segment offset, nbytes) ranges:
+        arena offset = segment offset, so the plan lines up with the saves' arena image."""
+        stager = self._stager_for([t for t, _, _ in device_ranges])
+        prepared = stager.prepare_ranges(device_ranges, [], for_write=True)
         if stager._attached is None:
             stager.attach(self.shared_memory)
         if stream is None:
@@ -1721,16 +1751,13 @@ class SharedMemoryHandler:
 
     def _run_rollback(self, stager: _DeviceStager, plan, stream) -> Optional[Dict[str, float]]:
         """One scatter kernel from the arena image; None (nothing done) without one."""
-        t0 = time.perf_counter()
-        if not plan.restore_from_image_async(self.shared_memory.dma_address, stream):
+        stats = _timed_restore(stager.ctx, plan, lambda: plan.restore_from_image_async(
+            self.shared_memory.dma_address, stream))
+        if stats is None:
             return None
-        stager.ctx.restore_wait()
-        wall_ms = (time.perf_counter() - t0) * 1e3
-        _, scatter, _ = stager.ctx.restore_timings()
-        self.last_restore_stats = {"device_bytes": float(plan.payload_bytes), "fill_ms": 0.0,
-                                   "scatter_ms": scatter, "direct": 0.0, "staged": 0.0,
-                                   "wall_ms": wall_ms, "from_image": 1.0}
-        return dict(self.last_restore_stats)
+        stats.update(fill_ms=0.0, direct=0.0, staged=0.0, from_image=1.0)
+        self.last_restore_stats = stats
+        return dict(stats)
 
     def _run_restore_cooperative(self, stager: _DeviceStager, plan, stream, coop):
         """Each of the n local ranks fills 1/n of its arena from the segment (its own PCIe
@@ -1775,17 +1802,13 @@ class SharedMemoryHandler:
         if not direct and stager.ensure_arena(plan) == stager.ARENA_NONE:
             direct = True
         staged = not stager.pinned()  # e.g. a restarted trainer: bounce slots, no 16 GB pin
-        t0 = time.perf_counter()
-        plan.restore_async(self.shared_memory.dma_address, stream, direct=direct)
-        stager.ctx.restore_wait()
-        wall_ms = (time.perf_counter() - t0) * 1e3
-        fill, scatter, _ = stager.ctx.restore_timings()
-        self.last_restore_stats = {"device_bytes": float(plan.payload_bytes), "fill_ms": fill,
-                                   "scatter_ms": scatter, "direct": float(direct),
-                                   "staged": float(staged), "wall_ms": wall_ms}
+        stats = _timed_restore(stager.ctx, plan, lambda: plan.restore_async(
+            self.shared_memory.dma_address, stream, direct=direct))
+        stats.update(direct=float(direct), staged=float(staged))
+        self.last_restore_stats = stats
         if pin_after:
             stager.pin_in_background()  # the next save wants plain DMA
-        return dict(self.last_restore_stats)
+        return dict(stats)
 
     def read_ranges(self, device_ranges, stream=None) -> Dict[str, float]:
         """Inverse of write_ranges for CUDA targets: (tensor, segment offset,
@@ -1802,13 +1825,7 @@ class SharedMemoryHandler:
                 raise ValueError("read_ranges needs CUDA targets")
             if off + nbytes > self.shared_memory.size or t.numel() * t.element_size() != nbytes:
                 raise ValueError("read_ranges: range does not fit the segment / the tensor")
-        stager = self._stager_for([r[0] for r in device_ranges])
-        prepared = stager.prepare_ranges(device_ranges, [], for_write=True)
-        if stager._attached is None:
-            stager.attach(self.shared_memory)
-        if stream is None:
-            stream = torch.cuda.current_stream(stager.device_index)
-        plan = stager.plan_for(prepared, role="restore", stream=stream)
+        stager, plan, stream = self._restore_plan(device_ranges, stream)
         return self._run_restore(stager, plan, stream)
 
     # -- queries ------------------------------------------------------------------------
@@ -1872,47 +1889,6 @@ def _pair_rows(src, dst):
     return out
 
 
-def _file_targets(index, target, strict: bool):
-    """Pair every tensor leaf of `target` with its TensorLeaf in the file: the tree rules
-    of restore_into (key strictness, exact shape and dtype, non-tensor leaves ignored).
-    Returns [(path, target tensor, leaf)] without 0-element leaves."""
-    from .torch_file_index import TensorLeaf
-
-    pairs = []
-
-    def walk(tgt, src, path):
-        if isinstance(src, Mapping):
-            if not isinstance(tgt, Mapping):
-                raise KeyError(f"{path}: checkpoint has a dict, target has {type(tgt).__name__}")
-            for k, s in src.items():
-                if k not in tgt:
-                    if strict:
-                        raise KeyError(f"{path}{k}: missing in target")
-                    continue
-                walk(tgt[k], s, f"{path}{k}.")
-            if strict:
-                extra = [k for k in tgt if k not in src]
-                if extra:
-                    raise KeyError(f"{path}: target keys not in checkpoint: {extra}")
-        elif isinstance(src, (list, tuple)):
-            if not isinstance(tgt, (list, tuple)) or len(tgt) != len(src):
-                raise KeyError(f"{path}: list length/type mismatch")
-            for i, s in enumerate(src):
-                walk(tgt[i], s, f"{path}{i}.")
-        elif isinstance(src, TensorLeaf):
-            name = path[:-1]
-            if not torch.is_tensor(tgt):
-                raise KeyError(f"{name}: checkpoint has a tensor, target has {type(tgt).__name__}")
-            if tuple(tgt.shape) != src.shape or tgt.dtype != src.dtype:
-                raise ValueError(f"{name}: shape/dtype mismatch {tuple(tgt.shape)}/{tgt.dtype} "
-                                 f"vs {src.shape}/{src.dtype}")
-            if src.numel:
-                pairs.append((name, tgt, src))
-
-    walk(target, index.tree, "")
-    return pairs
-
-
 def _file_ranges(index, pairs):
     """(target address, file offset, nbytes, leaf path) of every leaf of `pairs`, sorted by
     file offset.  A range that repeats bytes of another one into the same place (tied
@@ -1961,28 +1937,6 @@ def _disjoint_groups(ranges):
     return groups
 
 
-def _file_arena(ctx: native.Context, plan: native.Plan):
-    """Room for the plan in the arena; when HBM has none, a small arena through which the
-    library streams the plan window by window."""
-    end = plan.arena_end
-    if end <= ctx.arena_info()[1]:
-        return
-    forced = int(os.getenv("DLROVER_B200_ARENA_LIMIT_MB", "0") or 0)
-    if forced:
-        limit = max(8, forced) << 20
-        ctx.set_arena_limit(limit)
-        ctx.arena_reserve(min(end, limit))
-        return
-    try:
-        ctx.arena_reserve(end)
-    except native.NativeError as e:
-        if e.code != native.FC_ENOMEM:
-            raise
-        logger.warning(f"No room for a {end / 2**30:.1f} GiB restore arena in HBM: the file "
-                       "is restored window by window.")
-        ctx.arena_reserve(64 << 20)
-
-
 def _pread_into(fd: int, address: int, nbytes: int, offset: int):
     import ctypes
 
@@ -2009,12 +1963,12 @@ def restore_file_into(path: str, target, stream=None, strict: bool = True,
 
     Replaces `sd = torch.load(path, map_location="cpu"); model.load_state_dict(sd)`.
     stats: device_bytes, host_bytes, read_ms, scatter_ms, wall_ms."""
-    from .torch_file_index import index_file
+    from .torch_file_index import TensorLeaf, index_file
 
     t0 = time.perf_counter()
     if index is None:
         index = index_file(path)
-    pairs = _file_targets(index, target, strict)
+    pairs = _match_tree(target, index.tree, TensorLeaf, (list, tuple), strict)
     dev_pairs = [p for p in pairs if p[1].is_cuda]
     host_pairs = [p for p in pairs if not p[1].is_cuda]
     stats = {"device_bytes": 0.0, "host_bytes": 0.0, "read_ms": 0.0, "scatter_ms": 0.0,
@@ -2057,15 +2011,19 @@ def restore_file_into(path: str, target, stream=None, strict: bool = True,
                         a += n
                     plan = ctx.plan(ptrs, arena, lens, host_offsets=foffs)
                     try:
-                        _file_arena(ctx, plan)
-                        plan.restore_file_async(fd, stream)
-                        ctx.restore_wait()
-                        fill, scatter, _ = ctx.restore_timings()
+                        if (_DeviceStager.reserve_arena(ctx, plan.arena_end)
+                                == _DeviceStager.ARENA_NONE):
+                            logger.warning(f"No room for a {plan.arena_end / 2**30:.1f} GiB "
+                                           "restore arena in HBM: the file is restored window "
+                                           "by window.")
+                            ctx.arena_reserve(64 << 20)
+                        got = _timed_restore(ctx, plan,
+                                             lambda: plan.restore_file_async(fd, stream))
                     finally:
                         plan.destroy()
-                    stats["device_bytes"] += float(plan.payload_bytes)
-                    stats["read_ms"] += fill
-                    stats["scatter_ms"] += scatter
+                    stats["device_bytes"] += got["device_bytes"]
+                    stats["read_ms"] += got["fill_ms"]
+                    stats["scatter_ms"] += got["scatter_ms"]
             t1 = time.perf_counter()
             for p, f, n, _ in host:
                 _pread_into(fd, p, n, f)

@@ -22,6 +22,10 @@ model.
 """
 
 import contextlib
+import ctypes
+import mmap
+import os
+import time
 
 import numpy as np
 import pytest
@@ -510,21 +514,37 @@ class World:
                 self.arena[r.aoff - abase:r.aoff - abase + r.n] = data
         self._forget()
 
-    def restore(self, name="Q", host="A"):
+    def restore(self, name="Q", host="A", source="segment", src=None):
+        """Restore plan `name` from the bytes host buffer `host` holds, read from
+        `source`: "segment" (at address `src`, the buffer itself when None), "direct"
+        (the same, straight into the tensors), "file" (the open descriptor `src`) or
+        "image" (the arena image of the last save).  Returns the DMA copies it issued."""
         p = self.plans[name]
-        p["plan"].restore_async(self.host_t[host].data_ptr(), torch.cuda.current_stream())
+        plan, stream = p["plan"], torch.cuda.current_stream()
+        addr = self.host_t[host].data_ptr() if src is None else src
+        _, m0 = self.ctx.launch_count()
+        if source == "file":
+            plan.restore_file_async(src, stream)
+        elif source == "image":
+            assert plan.restore_from_image_async(addr, stream)
+        else:
+            plan.restore_async(addr, stream, direct=source == "direct")
         self.ctx.restore_wait()
         torch.cuda.synchronize()
-        if self.bounded:
+        _, m1 = self.ctx.launch_count()
+        if self.bounded or source == "direct":
             b = self.buf(name)
             for r in p["ranges"]:
                 b.np[r.tptr - b.base:r.tptr - b.base + r.n] = self.host[host][r.hoff:r.hoff + r.n]
         else:
             lo = self.arena_lo
-            for r in p["runs"]:
-                self.arena[r.aoff - lo:r.aoff - lo + r.n] = self.host[host][r.hoff:r.hoff + r.n]
+            if source != "image":
+                for r in p["runs"]:
+                    self.arena[r.aoff - lo:r.aoff - lo + r.n] = self.host[host][r.hoff:r.hoff + r.n]
             self._scatter(name)
-        self._forget()
+        if source != "image":  # a rollback keeps the baseline
+            self._forget()
+        return m1 - m0
 
     def arena_fill(self, host="A"):
         hi = self.lay.arena_end
@@ -672,6 +692,71 @@ def test_copy_kernels_write_exactly_the_covered_bytes(cuda_device, shape, varian
     # the copy ring and the byte-shift ring each wrap three times on a CTA that crosses
     # from item to item (the bulk tiles at chunk 4096, the shift tiles at 64 KiB and up)
     assert ring_tiles[0] >= 3 * stages and ring_tiles[1] >= 3 * shift_stages, ring_tiles
+
+
+@contextlib.contextmanager
+def _plain_mapping(data):
+    """The bytes of `data` in an anonymous mapping: pageable memory CUDA knows nothing of."""
+    mm = mmap.mmap(-1, data.size)
+    view = np.frombuffer(mm, dtype=np.uint8)
+    view[:] = data
+    anchor = ctypes.c_char.from_buffer(mm)
+    try:
+        yield ctypes.addressof(anchor)
+    finally:
+        del view, anchor
+        mm.close()
+
+
+@gpu
+@pytest.mark.parametrize("variant", VARIANTS, ids=["lsu", "tma"])
+@pytest.mark.parametrize("layout", ["state_dict", "mixed"])
+def test_every_restore_source_writes_exactly_the_target_bytes(cuda_device, tmp_path, layout,
+                                                              variant):
+    """Restores of one saved checkpoint from every source: the pinned segment, a plain
+    mapping (bounce slots), a mapping registered slice by slice, in place, a file and the
+    arena image; into the full arena and, where the source allows it, through an 8 MiB
+    one."""
+    lay = (state_dict_layout(9) if layout == "state_dict"
+           else mixed_layout(9, _tiles("default"), DEFAULT_CHUNK))
+    for bounded in (False, True):
+        lay.tgt.write(lay.tgt.base, pattern(lay.tgt.np.size))
+        ctx = _context("default", variant, 8 << 20 if bounded else 0)
+        ctx.set_stage(3, 1 << 20)
+        with _world(ctx, lay, 0, variant, bounded=bounded) as w:
+            assert (ctx.arena_info()[1] < lay.arena_end) == bounded
+            w.save()
+            w.check(f"save bounded={bounded}")
+            q, host = w.plans["Q"], w.host["A"]
+
+            def restore(source, src=None):
+                lay.tgt.write(lay.tgt.base, pattern(lay.tgt.np.size))
+                copies = w.restore(source=source, src=src)
+                w.check(f"{source} restore at {src} bounded={bounded}")
+                return copies
+
+            if not bounded:  # first: every other restore forgets the image
+                assert restore("image") == 0
+            copies = restore("segment")
+            if not bounded:
+                assert copies == pm.dma_count(q["runs"], 256 << 20)
+            assert restore("direct") >= q["plan"].n_spans
+            with _plain_mapping(host) as addr:
+                restore("segment", addr)
+                ctx.host_register_background(addr, host.size, slice_bytes=2 << 20)
+                deadline = time.time() + 60
+                while not ctx.host_ready(addr):
+                    assert time.time() < deadline
+                    time.sleep(0.01)
+                restore("segment", addr)
+                ctx.host_unregister(addr)
+            path = tmp_path / f"segment_{bounded}.bin"
+            path.write_bytes(host.tobytes())
+            fd = os.open(path, os.O_RDONLY)
+            try:
+                restore("file", fd)
+            finally:
+                os.close(fd)
 
 
 # --------------------------------------------------------- exact incremental accounting --
