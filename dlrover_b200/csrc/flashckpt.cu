@@ -12,8 +12,9 @@
 //      algorithmic traffic 2*S bytes per save;
 //   3. the arena is drained to the (pinned, NUMA-local) POSIX shm segment by DMA
 //      on a side stream gated by an event — the training stream only ever waits
-//      for (2).  A pump thread feeds the copy engine ONE 32 MiB piece at a time
-//      so the drain does not starve the application's own D2H copies;
+//      for (2).  A pump thread feeds the copy engine one kDrainPiece (16 MiB)
+//      piece at a time (fc_set_drain) so the drain does not starve the
+//      application's own D2H copies;
 //   4. restore is the inverse: DMA fill + scatter kernel;
 //   5. if the state does not fit in HBM a second time it is drained IN PLACE (DMA
 //      straight from the tensors, optionally with a snapshot of the tail that fits:
@@ -29,8 +30,8 @@
 //   fc_copy_tma_shift ranges whose source and destination are NOT congruent
 //                     mod 16: TMA in, funnel shift shared->shared, TMA out.
 //   fc_copy_lsu       256-thread CTAs, 128-bit LDG/STG, 4-way unrolled: heads,
-//                     tails, tiny ranges, the bounded-arena windows, and
-//                     everything when FC_VARIANT_LSU is selected.
+//                     tails, tiny ranges, and everything when FC_VARIANT_LSU is
+//                     selected.
 // and, for the opt-in incremental save (fc_save_delta_async), their gather-compare
 // twins fc_delta_tma / fc_delta_lsu: they write only the bytes that differ from the
 // arena's previous image and mark the work items to drain.
@@ -117,6 +118,14 @@ struct DeltaMap {
   }
 };
 
+// One part of a transfer between the device and the host: len bytes at device address dev,
+// at offset off of the host mapping (or of the file a restore reads).
+struct Seg {
+  uint8_t* dev;
+  uint64_t off;
+  uint64_t len;
+};
+
 struct fc_ctx {
   int device = 0;
   int sm_count = 132;
@@ -172,10 +181,9 @@ struct fc_ctx {
   struct DrainJob {
     int staged_threads = 0;  // > 0: host range not registered, go through the bounce slots
     uint8_t* host = nullptr;
-    std::vector<FcRun> runs;
-    std::vector<FcSpan> spans;  // in-place save: DMA straight from the tensors
-    bool direct = false;
-    uint64_t arena_base = 0;  // arena byte 0 holds this segment offset (hybrid: the cut)
+    std::vector<Seg> spans;  // in-place part: DMA straight from the tensors, drained first
+    std::vector<Seg> runs;   // arena part
+    bool direct = false;     // in-place form: report the in-place part (inplace_done_ticket)
     uint64_t ticket = 0;
     // incremental save: `runs` is built by the pump from the items marked `seq`
     std::shared_ptr<const DeltaMap> delta;
@@ -288,12 +296,16 @@ struct StagePiece {
   uint64_t foff;  // file offset when the source is a file (StageFile), else unused
 };
 
-// Cuts a transfer of len bytes into slot-sized pieces.  host == nullptr: the bytes are read
-// from a file at offset foff.
-static void stage_pieces(std::vector<StagePiece>& out, uint8_t* dev, uint8_t* host, uint64_t len,
-                         uint64_t slot, uint64_t foff = 0) {
-  for (uint64_t o = 0; o < len; o += slot)
-    out.push_back({dev + o, host ? host + o : nullptr, std::min<uint64_t>(slot, len - o), foff + o});
+// Cuts every segment into slot-sized pieces.  host == nullptr: the segments' offsets are
+// file offsets.
+static std::vector<StagePiece> stage_pieces(const std::vector<Seg>& segs, uint8_t* host,
+                                            uint64_t slot) {
+  std::vector<StagePiece> out;
+  for (const Seg& g : segs)
+    for (uint64_t o = 0; o < g.len; o += slot)
+      out.push_back({g.dev + o, host ? host + g.off + o : nullptr,
+                     std::min<uint64_t>(slot, g.len - o), g.off + o});
+  return out;
 }
 
 // A file as the source of a staged fill (fc_restore_file_async): the workers pread each
@@ -432,16 +444,133 @@ static cudaError_t delta_runs(fc_ctx* c, fc_ctx::DrainJob& job) {
     if (c->dirty_pinned[i] != job.seq) continue;
     while (m.runs[r].off + m.runs[r].len <= m.aoff[i]) ++r;
     const uint64_t hoff = m.runs[r].hoff + (m.aoff[i] - m.runs[r].off);
+    uint8_t* dev = c->arena + m.aoff[i];
     if (!job.runs.empty()) {
-      FcRun& last = job.runs.back();
-      if (last.off + last.len == m.aoff[i] && last.hoff + last.len == hoff) {
+      Seg& last = job.runs.back();
+      if (last.dev + last.len == dev && last.off + last.len == hoff) {
         last.len += m.len[i];
         continue;
       }
     }
-    job.runs.push_back({m.aoff[i], m.len[i], hoff});
+    job.runs.push_back({dev, hoff, m.len[i]});
   }
   return cudaSuccess;
+}
+
+// Calls put(host destination, device source, length) for every piece of segs: at most
+// drain_piece bytes, never across a slice boundary of the host range.  Stops at the first
+// error.
+template <class Put>
+static cudaError_t for_pieces(fc_ctx* c, uint8_t* host, const std::vector<Seg>& segs,
+                              const SliceClip& clip, Put put) {
+  cudaError_t e = cudaSuccess;
+  for (const Seg& g : segs)
+    for (uint64_t o = 0, len = 0; o < g.len && e == cudaSuccess; o += len) {
+      len = clip(host + g.off + o, std::min<uint64_t>(c->drain_piece, g.len - o));
+      e = put(host + g.off + o, g.dev + o, len);
+    }
+  return e;
+}
+
+// The in-place part: one batch (<= drain_piece bytes, <= 64 copies) in flight, then wait:
+// the pacing rule of the arena part, and small tensors share a batch.
+static cudaError_t drain_spans(fc_ctx* c, uint8_t* host, const std::vector<Seg>& segs,
+                               const SliceClip& clip, uint64_t* copies) {
+  uint64_t batch_bytes = 0;
+  int batch_n = 0;
+  auto flush = [&] {
+    batch_bytes = 0;
+    batch_n = 0;
+    cudaError_t e = cudaEventRecord(c->ring[0], c->copy_stream);
+    return e == cudaSuccess ? cudaEventSynchronize(c->ring[0]) : e;
+  };
+  auto put = [&](uint8_t* dst, const uint8_t* src, uint64_t len) {
+    cudaError_t e = cudaMemcpyAsync(dst, src, len, cudaMemcpyDeviceToHost, c->copy_stream);
+    ++*copies;
+    batch_bytes += len;
+    if (e == cudaSuccess && (batch_bytes >= c->drain_piece || ++batch_n >= 64)) e = flush();
+    return e;
+  };
+  cudaError_t e = for_pieces(c, host, segs, clip, put);
+  if (e == cudaSuccess && batch_bytes) e = flush();
+  return e;
+}
+
+// The arena part: host-paced (piece k is submitted once piece k - drain_depth has
+// completed) or chained on the device (ping-pong mode).  On return copy_stream is ordered
+// after the last piece.
+static cudaError_t drain_runs(fc_ctx* c, uint8_t* host, const std::vector<Seg>& segs,
+                              const SliceClip& clip, uint64_t* copies) {
+  const int depth = std::max(1, std::min(c->drain_depth, kDrainRing));
+  const bool pingpong = c->drain_mode == FC_DRAIN_PINGPONG && c->copy_stream2 != nullptr;
+  cudaStream_t last_stream = c->copy_stream;
+  uint64_t k = 0;
+  auto put = [&](uint8_t* dst, const uint8_t* src, uint64_t len) {
+    cudaError_t e = cudaSuccess;
+    if (pingpong) {
+      // Piece k goes to stream k&1 and waits ON THE DEVICE for piece k-1 (the other
+      // stream): neither stream ever has a second copy queued behind the one in
+      // flight, so the copy engine arbitrates between our next piece and a
+      // foreign copy after every piece — and there is no host round trip between
+      // two pieces.  The host only keeps two pieces submitted.
+      cudaStream_t sk = (k & 1) ? c->copy_stream2 : c->copy_stream;
+      if (k >= 2) e = cudaEventSynchronize(c->ring_pp[(k - 2) % kDrainRing]);
+      if (e == cudaSuccess && k >= 1)
+        e = cudaStreamWaitEvent(sk, c->ring_pp[(k - 1) % kDrainRing], 0);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(dst, src, len, cudaMemcpyDeviceToHost, sk);
+      if (e == cudaSuccess) e = cudaEventRecord(c->ring_pp[k % kDrainRing], sk);
+      last_stream = sk;
+    } else {
+      if (k >= (uint64_t)depth) e = cudaEventSynchronize(c->ring[k % depth]);  // piece k-depth
+      if (e == cudaSuccess)
+        e = cudaMemcpyAsync(dst, src, len, cudaMemcpyDeviceToHost, c->copy_stream);
+      if (e == cudaSuccess) e = cudaEventRecord(c->ring[k % depth], c->copy_stream);
+    }
+    ++k;
+    ++*copies;
+    return e;
+  };
+  cudaError_t e = for_pieces(c, host, segs, clip, put);
+  if (e == cudaSuccess && last_stream != c->copy_stream)
+    e = cudaStreamWaitEvent(c->copy_stream, c->ring_pp[(k - 1) % kDrainRing], 0);
+  return e;
+}
+
+// One part of a drain job: through the bounce slots when the host range is not
+// page-locked, else by DMA under the part's pacing rule (drain_spans or drain_runs).
+using DmaDrain = cudaError_t (*)(fc_ctx*, uint8_t*, const std::vector<Seg>&, const SliceClip&,
+                                 uint64_t*);
+static cudaError_t drain_part(fc_ctx* c, const fc_ctx::DrainJob& job, const std::vector<Seg>& segs,
+                              DmaDrain dma, uint64_t* copies) {
+  if (job.staged_threads > 0) {
+    const std::vector<StagePiece> pieces = stage_pieces(segs, job.host, c->stage_slot);
+    *copies += pieces.size();
+    return stage_run(c, pieces, true, c->ev_pack_end, job.staged_threads);
+  }
+  // a range registered slice by slice: no DMA may straddle two slices
+  const SliceClip clip(c, job.host + (segs.empty() ? 0 : segs.front().off));
+  return dma(c, job.host, segs, clip, copies);
+}
+
+// Drains one save once its gather has completed: the in-place part first (then the
+// tensors are free again), then the arena part; ev_drain_start / ev_drain_end bracket it.
+static cudaError_t drain_job(fc_ctx* c, fc_ctx::DrainJob& job, uint64_t* copies) {
+  cudaError_t e = cudaStreamWaitEvent(c->copy_stream, c->ev_pack_end, 0);
+  if (e == cudaSuccess) e = cudaEventRecord(c->ev_drain_start, c->copy_stream);
+  if (job.delta && e == cudaSuccess) e = delta_runs(c, job);
+  if (e == cudaSuccess) e = drain_part(c, job, job.spans, drain_spans, copies);
+  if (job.direct) {
+    {
+      // the tensors are free again (on error too: nothing reads them any more)
+      std::lock_guard<std::mutex> lk(c->mu);
+      c->inplace_done_ticket = job.ticket;
+    }
+    c->cv.notify_all();
+  }
+  if (e == cudaSuccess) e = drain_part(c, job, job.runs, drain_runs, copies);
+  if (e == cudaSuccess) e = cudaEventRecord(c->ev_drain_end, c->copy_stream);
+  if (e == cudaSuccess) e = cudaEventSynchronize(c->ev_drain_end);
+  return e;
 }
 
 static void pump_main(fc_ctx* c) {
@@ -458,112 +587,11 @@ static void pump_main(fc_ctx* c) {
       job = std::move(c->jobs.front());
       c->jobs.pop_front();
     }
-    cudaError_t e = cudaStreamWaitEvent(c->copy_stream, c->ev_pack_end, 0);
-    if (e == cudaSuccess) e = cudaEventRecord(c->ev_drain_start, c->copy_stream);
-    if (job.delta && e == cudaSuccess) e = delta_runs(c, job);
+    uint64_t copies = 0;
+    const cudaError_t e = drain_job(c, job, &copies);
     uint64_t drained = 0;
-    for (const FcRun& r : job.runs) drained += r.len;
-    for (const FcSpan& sp : job.spans) drained += sp.len;
-    const bool delta = job.delta != nullptr;
-    const int depth = std::max(1, std::min(c->drain_depth, kDrainRing));
-    uint64_t k = 0, copies = 0;
-    if (job.staged_threads > 0 && e == cudaSuccess) {
-      // host range not registered: bounce through pinned slots (in-place part first)
-      std::vector<StagePiece> pieces;
-      for (const FcSpan& sp : job.spans)
-        stage_pieces(pieces, (uint8_t*)(uintptr_t)sp.tptr, job.host + sp.off, sp.len,
-                     c->stage_slot);
-      if (!pieces.empty()) {
-        e = stage_run(c, pieces, true, c->ev_pack_end, job.staged_threads);
-        copies += pieces.size();
-        pieces.clear();
-      }
-      if (job.direct) {
-        {
-          std::lock_guard<std::mutex> lk(c->mu);
-          c->inplace_done_ticket = job.ticket;
-        }
-        c->cv.notify_all();
-      }
-      for (const FcRun& r : job.runs)
-        stage_pieces(pieces, c->arena + (r.off - job.arena_base), job.host + r.hoff, r.len,
-                     c->stage_slot);
-      if (e == cudaSuccess) e = stage_run(c, pieces, true, c->ev_pack_end, job.staged_threads);
-      copies += pieces.size();
-      job.runs.clear();
-      job.direct = false;
-    }
-    // a range registered slice by slice: no DMA may straddle two slices
-    const uint64_t first_off = !job.runs.empty() ? job.runs.front().hoff
-                               : !job.spans.empty() ? job.spans.front().off : 0;
-    const SliceClip clip(c, job.host + first_off);
-    if (job.direct) {
-      // one batch (<= drain_piece bytes, <= 64 copies) in flight, then wait: same
-      // pacing rule as below, small tensors share a batch
-      uint64_t batch_bytes = 0;
-      int batch_n = 0;
-      for (const FcSpan& sp : job.spans) {
-        for (uint64_t o = 0, len = 0; o < sp.len && e == cudaSuccess; o += len) {
-          len = clip(job.host + sp.off + o, std::min<uint64_t>(c->drain_piece, sp.len - o));
-          e = cudaMemcpyAsync(job.host + sp.off + o, (const uint8_t*)(uintptr_t)sp.tptr + o, len,
-                              cudaMemcpyDeviceToHost, c->copy_stream);
-          ++copies;
-          batch_bytes += len;
-          if (e == cudaSuccess && (batch_bytes >= c->drain_piece || ++batch_n >= 64)) {
-            e = cudaEventRecord(c->ring[0], c->copy_stream);
-            if (e == cudaSuccess) e = cudaEventSynchronize(c->ring[0]);
-            batch_bytes = 0;
-            batch_n = 0;
-          }
-        }
-      }
-      if (e == cudaSuccess && (batch_bytes || batch_n)) {
-        e = cudaEventRecord(c->ring[0], c->copy_stream);
-        if (e == cudaSuccess) e = cudaEventSynchronize(c->ring[0]);
-      }
-      {
-        // the tensors are free again (on error too: nothing reads them any more)
-        std::lock_guard<std::mutex> lk(c->mu);
-        c->inplace_done_ticket = job.ticket;
-      }
-      c->cv.notify_all();
-    }
-    const bool pingpong = c->drain_mode == FC_DRAIN_PINGPONG && c->copy_stream2 != nullptr;
-    cudaStream_t last_stream = c->copy_stream;
-    for (const FcRun& r : job.runs) {
-      for (uint64_t o = 0, len = 0; o < r.len && e == cudaSuccess; o += len) {
-        uint8_t* dst = job.host + r.hoff + o;
-        len = clip(dst, std::min<uint64_t>(c->drain_piece, r.len - o));
-        const uint8_t* src = c->arena + (r.off - job.arena_base) + o;
-        if (pingpong) {
-          // Piece k goes to stream k&1 and waits ON THE DEVICE for piece k-1 (the other
-          // stream): neither stream ever has a second copy queued behind the one in
-          // flight, so the copy engine arbitrates between our next piece and a
-          // foreign copy after every piece — and there is no host round trip between
-          // two pieces.  The host only keeps two pieces submitted.
-          cudaStream_t sk = (k & 1) ? c->copy_stream2 : c->copy_stream;
-          if (k >= 2) e = cudaEventSynchronize(c->ring_pp[(k - 2) % kDrainRing]);
-          if (e == cudaSuccess && k >= 1)
-            e = cudaStreamWaitEvent(sk, c->ring_pp[(k - 1) % kDrainRing], 0);
-          if (e == cudaSuccess) e = cudaMemcpyAsync(dst, src, len, cudaMemcpyDeviceToHost, sk);
-          if (e == cudaSuccess) e = cudaEventRecord(c->ring_pp[k % kDrainRing], sk);
-          last_stream = sk;
-        } else {
-          if (k >= (uint64_t)depth) e = cudaEventSynchronize(c->ring[k % depth]);  // piece k-depth
-          if (e == cudaSuccess)
-            e = cudaMemcpyAsync(dst, src, len, cudaMemcpyDeviceToHost, c->copy_stream);
-          if (e == cudaSuccess) e = cudaEventRecord(c->ring[k % depth], c->copy_stream);
-        }
-        ++k;
-        ++copies;
-      }
-    }
-    if (e == cudaSuccess && last_stream != c->copy_stream) {
-      // ev_drain_end is recorded on copy_stream: order it after the last piece
-      e = cudaStreamWaitEvent(c->copy_stream, c->ring_pp[(k - 1) % kDrainRing], 0);
-    }
-    if (e == cudaSuccess) e = cudaEventRecord(c->ev_drain_end, c->copy_stream);
-    if (e == cudaSuccess) e = cudaEventSynchronize(c->ev_drain_end);
+    for (const Seg& g : job.spans) drained += g.len;
+    for (const Seg& g : job.runs) drained += g.len;
     {
       std::lock_guard<std::mutex> lk(c->mu);
       c->n_memcpys += copies;
@@ -579,7 +607,7 @@ static void pump_main(fc_ctx* c) {
       }
       c->stat_ticket = job.ticket;
       c->stat_bytes = drained;
-      c->stat_delta = delta ? 1 : 0;
+      c->stat_delta = job.delta ? 1 : 0;
       c->drained_ticket = job.ticket;
     }
     c->cv.notify_all();
@@ -1592,10 +1620,11 @@ extern "C" int fc_unpack_async(fc_plan* p, void* stream, int variant) {
 // When the state does not fit a second time in HBM (arena smaller than the
 // plan: fc_set_arena_limit, or the full-size cudaMalloc failed) the checkpoint is
 // streamed through the arena window by window: gather the items of one window
-// (LSU kernel over a slice of the offset-sorted table), DMA the window's bytes,
-// next window.  The tensors must not change until the LAST window has been
+// (the plan's kernels over a slice of the offset-sorted table), DMA the window's
+// bytes, next window.  The tensors must not change until the LAST window has been
 // gathered, so this mode blocks the caller for the whole checkpoint — the
-// reference's behaviour, at PCIe instead of pageable-copy speed.
+// reference's behaviour, at PCIe instead of pageable-copy speed.  Restores stream
+// the same windows the other way.
 struct Window {
   uint32_t i0, i1;      // item index range in h_all / d_all
   uint64_t base, end;   // segment byte range covered
@@ -1612,60 +1641,11 @@ static std::vector<Window> make_windows(const fc_plan* p, uint64_t arena_bytes) 
       cur.end = std::max<uint64_t>(cur.end, it[cur.i1].aoff + it[cur.i1].nbytes);
       ++cur.i1;
     }
-    if (cur.i1 == cur.i0) return {};  // one item larger than the arena: cannot happen (>= 8 MiB)
+    if (cur.i1 == cur.i0) return {};  // one item larger than the arena
     w.push_back(cur);
     i = cur.i1;
   }
   return w;
-}
-
-// Drain the parts of the plan's runs that fall into [lo, hi), one piece at a time.
-static int copy_window(fc_ctx* c, const fc_plan* p, uint8_t* host, uint64_t lo, uint64_t hi,
-                       uint64_t base) {
-  const SliceClip clip(c, host + lo);
-  for (const FcRun& r : p->runs) {
-    uint64_t a = std::max(lo, r.off), b = std::min(hi, r.off + r.len);
-    for (uint64_t o = a, len = 0; o < b; o += len) {
-      len = clip(host + o, std::min<uint64_t>(c->drain_piece, b - o));
-      FC_CUDA(cudaMemcpyAsync(host + o, c->arena + (o - base), len, cudaMemcpyDeviceToHost,
-                              c->copy_stream));
-      c->n_memcpys += 1;
-      FC_CUDA(cudaStreamSynchronize(c->copy_stream));  // paced: one piece in flight
-    }
-  }
-  return FC_OK;
-}
-
-static int save_windowed(fc_plan* p, uint8_t* host, cudaStream_t cs) {
-  fc_ctx* c = p->ctx;
-  std::vector<Window> wins = make_windows(p, c->arena_bytes);
-  if (wins.empty() && !p->h_all.empty())
-    return fail(FC_EINVAL, "arena window too small for a work item%s%s");
-  FC_CUDA(cudaStreamWaitEvent(cs, p->ev_upload, 0));
-  FC_CUDA(cudaEventRecord(c->ev_pack_start, cs));
-  bool first = true;
-  for (const Window& w : wins) {
-    int rc = launch_slice<0>(p, cs, FC_VARIANT_AUTO, w.i0, w.i1, w.abase);
-    if (rc) return rc;
-    FC_CUDA(cudaEventRecord(c->ev_pack_end, cs));
-    FC_CUDA(cudaStreamWaitEvent(c->copy_stream, c->ev_pack_end, 0));
-    if (first) {
-      FC_CUDA(cudaEventRecord(c->ev_drain_start, c->copy_stream));
-      first = false;
-    }
-    rc = copy_window(c, p, host, w.base, w.end, w.abase);
-    if (rc) return rc;
-    // the next gather overwrites the window: it must wait for this drain
-    FC_CUDA(cudaEventRecord(c->ev_drain_end, c->copy_stream));
-    FC_CUDA(cudaStreamWaitEvent(cs, c->ev_drain_end, 0));
-  }
-  if (first) FC_CUDA(cudaEventRecord(c->ev_drain_start, c->copy_stream));
-  FC_CUDA(cudaEventRecord(c->ev_pack_end, cs));
-  FC_CUDA(cudaEventRecord(p->ev_last_use, cs));
-  FC_CUDA(cudaEventRecord(c->ev_drain_end, c->copy_stream));
-  FC_CUDA(cudaEventSynchronize(c->ev_drain_end));
-  FC_CUDA(cudaEventSynchronize(c->ev_pack_end));
-  return FC_OK;
 }
 
 // ---- restores ---------------------------------------------------------------------
@@ -1683,13 +1663,6 @@ static int restore_begin(fc_ctx* c, const char* busy, bool forget = true) {
   return FC_OK;
 }
 
-// One part of a fill: len bytes to device address dev from offset src of the source.
-struct FillSeg {
-  uint8_t* dev;
-  uint64_t src;
-  uint64_t len;
-};
-
 // Where a fill reads: the host mapping `host`, or the file `file` (host unused).
 struct FillSource {
   const uint8_t* host;
@@ -1697,24 +1670,23 @@ struct FillSource {
   const char* what;  // prefix of the error a failed staged copy returns
 };
 
-// Moves every segment's bytes from src.  A file, or a host range that is not page-locked,
-// goes through the bounce slots (the stage workers start once `gate`, if any, has
-// completed) and is on the device on return.  A page-locked range is queued on the copy
-// stream in kDmaPiece pieces cut at slice boundaries.
-static int restore_fill(fc_ctx* c, const std::vector<FillSeg>& segs, const FillSource& src,
+// Moves every segment's bytes from src (Seg::off: offset in the source).  A file, or a
+// host range that is not page-locked, goes through the bounce slots (the stage workers
+// start once `gate`, if any, has completed) and is on the device on return.  A page-locked
+// range is queued on the copy stream in kDmaPiece pieces cut at slice boundaries.
+static int restore_fill(fc_ctx* c, const std::vector<Seg>& segs, const FillSource& src,
                         cudaEvent_t gate) {
   if (segs.empty()) return FC_OK;
   uint64_t lo = ~0ull, hi = 0;
-  for (const FillSeg& g : segs) {
-    lo = std::min(lo, g.src);
-    hi = std::max(hi, g.src + g.len);
+  for (const Seg& g : segs) {
+    lo = std::min(lo, g.off);
+    hi = std::max(hi, g.off + g.len);
   }
   uint8_t* host = const_cast<uint8_t*>(src.host);
   const int staged = src.file ? c->stage_threads : staged_threads_for(c, host + lo, hi - lo);
   if (staged > 0) {
-    std::vector<StagePiece> pieces;
-    for (const FillSeg& g : segs)
-      stage_pieces(pieces, g.dev, src.file ? nullptr : host + g.src, g.len, c->stage_slot, g.src);
+    const std::vector<StagePiece> pieces = stage_pieces(segs, src.file ? nullptr : host,
+                                                        c->stage_slot);
     cudaError_t e = stage_run(c, pieces, false, gate, staged, src.file);
     if (src.file && src.file->failed.load()) {
       char at[64];
@@ -1727,10 +1699,10 @@ static int restore_fill(fc_ctx* c, const std::vector<FillSeg>& segs, const FillS
     return FC_OK;
   }
   const SliceClip clip(c, host + lo);
-  for (const FillSeg& g : segs)
+  for (const Seg& g : segs)
     for (uint64_t o = 0, len = 0; o < g.len; o += len) {
-      len = clip(host + g.src + o, std::min<uint64_t>(kDmaPiece, g.len - o));
-      FC_CUDA(cudaMemcpyAsync(g.dev + o, host + g.src + o, len, cudaMemcpyHostToDevice,
+      len = clip(host + g.off + o, std::min<uint64_t>(kDmaPiece, g.len - o));
+      FC_CUDA(cudaMemcpyAsync(g.dev + o, host + g.off + o, len, cudaMemcpyHostToDevice,
                               c->copy_stream));
       c->n_memcpys += 1;
     }
@@ -1740,7 +1712,7 @@ static int restore_fill(fc_ctx* c, const std::vector<FillSeg>& segs, const FillS
 // A fill into memory that work queued on `s` may still use (the tensors of an in-place
 // restore, the arena of fc_arena_fill): it starts once `s` has reached this point, and
 // `s` continues once the bytes are in place.
-static int restore_fill_gated(fc_ctx* c, cudaStream_t s, const std::vector<FillSeg>& segs,
+static int restore_fill_gated(fc_ctx* c, cudaStream_t s, const std::vector<Seg>& segs,
                               const FillSource& src) {
   FC_CUDA(cudaEventRecord(c->ev_scatter_end, s));
   FC_CUDA(cudaStreamWaitEvent(c->copy_stream, c->ev_scatter_end, 0));
@@ -1753,8 +1725,8 @@ static int restore_fill_gated(fc_ctx* c, cudaStream_t s, const std::vector<FillS
 }
 
 // The plan's runs inside arena range [lo, hi), into an arena whose byte 0 stands for offset ab.
-static std::vector<FillSeg> run_segs(const fc_plan* p, uint64_t lo, uint64_t hi, uint64_t ab) {
-  std::vector<FillSeg> segs;
+static std::vector<Seg> run_segs(const fc_plan* p, uint64_t lo, uint64_t hi, uint64_t ab) {
+  std::vector<Seg> segs;
   for (const FcRun& r : p->runs) {
     const uint64_t a = std::max(lo, r.off), b = std::min(hi, r.off + r.len);
     if (a < b) segs.push_back({p->ctx->arena + (a - ab), r.hoff + (a - r.off), b - a});
@@ -1813,16 +1785,289 @@ static int restore_arena(fc_plan* p, cudaStream_t s, const FillSource* src) {
   return FC_OK;
 }
 
-static int save_async_impl(fc_plan* p, void* host_base, void* compute_stream, uint64_t* ticket,
-                           bool hold);
+// ---- saves ------------------------------------------------------------------------
+// Every save is one form of the same thing: the plan's ranges below segment offset `cut`
+// drain in place (DMA straight from the tensors, first), the ranges from the cut on are
+// gathered into the arena, whose byte 0 stands for the cut rounded down to 128 B, and
+// drained from there.  cut = 0 snapshots everything (fc_save_async, fc_save_delta_async),
+// cut = ~0 drains everything in place (fc_save_direct_async), anything else is a hybrid
+// (fc_save_hybrid_async).  Each save runs the same checks (save_begin), one gather
+// (save_gather) and one enqueue (save_enqueue); the pump drains it (drain_job).  A save
+// through a bounded arena is drained window by window on the caller's thread instead
+// (save_windowed).
+struct SaveForm {
+  const char* who;   // prefix of the refusals
+  uint64_t cut;
+  bool in_place;     // fc_save_hybrid_async / fc_save_direct_async: identity and cut rules,
+                     // the sources stay frozen until the in-place part drained, no image
+  bool incremental;  // fc_save_delta_async: compare with the baseline, then become it
+  bool hold;         // the drain waits for fc_save_release
+};
 
+static int launch_delta_lsu(fc_ctx* c, const FcItem* items, uint32_t n, cudaStream_t s,
+                            uint32_t seq) {
+  if (n == 0) return FC_OK;
+  uint32_t grid = std::min<uint32_t>(n, (uint32_t)(c->sm_count * c->lsu_ctas_per_sm));
+  fc_delta_lsu<<<grid, kLsuThreads, 0, s>>>(items, n, c->arena, c->dirty, seq);
+  FC_CUDA(cudaGetLastError());
+  c->n_kernels += 1;
+  return FC_OK;
+}
+
+// The ring takes the copy ring's shared memory (fc_set_launch): a stage holds a source
+// and an old tile of half the copy tile each (default 2 stages x 2 x 48 KiB).
+static int launch_delta_tma(fc_ctx* c, const FcItem* items, uint32_t n, cudaStream_t s,
+                            uint32_t seq) {
+  if (n == 0) return FC_OK;
+  const uint32_t tile = std::max<uint32_t>(128u, ((uint32_t)c->tma_tile / 2u) & ~127u);
+  const uint32_t stages = (uint32_t)c->tma_stages;
+  const size_t smem = delta_smem_bytes(tile, stages);
+  FC_CUDA(cudaFuncSetAttribute(fc_delta_tma, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)smem));
+  uint32_t grid = std::min<uint32_t>(n, (uint32_t)(c->sm_count * c->tma_ctas_per_sm));
+  fc_delta_tma<<<grid, kDeltaThreads, smem, s>>>(items, n, c->arena, c->dirty, seq, tile, stages);
+  FC_CUDA(cudaGetLastError());
+  c->n_kernels += 1;
+  return FC_OK;
+}
+
+// Gather-compare over the whole plan: bulk bodies through the TMA ring, shifted ranges
+// and residues through the LSU kernel (FC_VARIANT_LSU: every item through the LSU kernel).
+static int launch_delta(fc_plan* p, cudaStream_t s, uint32_t seq) {
+  fc_ctx* c = p->ctx;
+  if (c->variant != FC_VARIANT_TMA) return launch_delta_lsu(c, p->all.dev, p->all.n, s, seq);
+  int rc = launch_delta_tma(c, p->bulk.dev, p->bulk.n, s, seq);
+  if (!rc) rc = launch_delta_lsu(c, p->shift.dev, p->shift.n, s, seq);
+  if (!rc) rc = launch_delta_lsu(c, p->resid.dev, p->resid.n, s, seq);
+  return rc;
+}
+
+// What a save covers once its checks have passed.
+struct SaveScope {
+  uint32_t i0 = 0;          // first item of the arena part
+  uint64_t abase = 0;       // segment offset arena byte 0 stands for
+  std::vector<Window> wins; // a bounded-arena save: its windows
+};
+
+// The checks of a save after the null argument, in a fixed order: the busy rule, the
+// form's own rules, the sticky drain error.  Nothing is forgotten or written before all of
+// them have passed.
+static int save_begin(fc_plan* p, const SaveForm& f, SaveScope* s) {
+  fc_ctx* c = p->ctx;
+  int rc = refresh_inflight(c);
+  if (rc) return rc;
+  if (c->save_inflight || c->restore_inflight)
+    return fail(FC_EBUSY, "%s: previous save/restore still draining%s", f.who);
+  if (f.in_place) {
+    if (!p->identity && f.cut != ~0ull)
+      return fail(FC_EINVAL, "fc_save_hybrid_async: needs a plan whose arena is an image of "
+                             "the segment%s%s");
+    const std::vector<FcItem>& it = p->h_all;
+    s->i0 = (uint32_t)(std::lower_bound(it.begin(), it.end(), f.cut,
+                                        [](const FcItem& a, uint64_t v) { return a.aoff < v; }) -
+                       it.begin());
+    if (s->i0 > 0 && it[s->i0 - 1].aoff + it[s->i0 - 1].nbytes > f.cut)
+      return fail(FC_EINVAL, "fc_save_hybrid_async: cut is not a tensor boundary%s%s");
+    s->abase = arena_base_for(std::min(f.cut, p->arena_end));
+    if (s->i0 < it.size() && p->arena_end - s->abase > c->arena_bytes)
+      return fail(FC_EINVAL, "fc_save_hybrid_async: arena smaller than the snapshot part%s%s");
+  } else if (p->arena_end > c->arena_bytes) {
+    if (f.incremental)
+      return fail(FC_EINVAL, "fc_save_delta_async: the arena must hold the whole plan (no "
+                             "incremental bounded-arena save)%s%s");
+    if (c->arena_bytes < (8ull << 20) || !p->identity)
+      return fail(FC_EINVAL, "arena smaller than the plan: call fc_arena_reserve first%s%s");
+    s->wins = make_windows(p, c->arena_bytes);
+    if (s->wins.empty()) return fail(FC_EINVAL, "arena window too small for a work item%s%s");
+  }
+  // a sticky drain error must surface BEFORE the arena is overwritten
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (c->drain_rc != FC_OK) return fail(c->drain_rc, "%s", c->drain_err.c_str());
+  return FC_OK;
+}
+
+// The gather of a save on the caller's stream, between ev_pack_start and ev_pack_end: the
+// copy kernels over the items from i0 on, or (compare) the gather-compare kernels over
+// the whole plan.  With no item the pair of events still orders the drain after
+// everything already queued on the stream (the optimizer step that produced the values).
+static int save_gather(fc_plan* p, cudaStream_t cs, const SaveScope& s, bool compare) {
+  fc_ctx* c = p->ctx;
+  const uint32_t n = p->all.n;
+  if (compare) {
+    bool reset = false;
+    if (n > c->dirty_cap) {
+      const uint32_t cap = (uint32_t)std::min<uint64_t>(0xFFFFFFF0ull, n + n / 4 + 16);
+      uint32_t* nd = nullptr;
+      uint32_t* np = nullptr;
+      cudaError_t e = cudaMalloc(&nd, (size_t)cap * sizeof(uint32_t));
+      if (e == cudaSuccess)
+        e = cudaHostAlloc(&np, (size_t)cap * sizeof(uint32_t), cudaHostAllocDefault);
+      if (e != cudaSuccess) {
+        (void)cudaGetLastError();
+        if (nd) c->dead_dev.push_back(nd);
+        return fail(FC_ENOMEM, "dirty marks alloc: %s", cudaGetErrorString(e));
+      }
+      if (c->dirty) c->dead_dev.push_back(c->dirty);  // no save is in flight: nothing reads them
+      if (c->dirty_pinned) c->dead_pinned.push_back(c->dirty_pinned);
+      c->dirty = nd;
+      c->dirty_pinned = np;
+      c->dirty_cap = cap;
+      reset = true;
+    }
+    // marks are sequence numbers: cleared only for a fresh array or when seq wraps
+    if (++c->delta_seq == 0) reset = true;
+    if (reset) {
+      FC_CUDA(cudaMemsetAsync(c->dirty, 0, (size_t)c->dirty_cap * sizeof(uint32_t), cs));
+      c->delta_seq = 1;
+    }
+  }
+  FC_CUDA(cudaEventRecord(c->ev_pack_start, cs));
+  if (s.i0 < n) {
+    FC_CUDA(cudaStreamWaitEvent(cs, p->ev_upload, 0));  // tables may come from another stream
+    int rc = compare ? launch_delta(p, cs, c->delta_seq)
+                     : launch_slice<0>(p, cs, FC_VARIANT_AUTO, s.i0, n, s.abase);
+    if (rc) return rc;
+    FC_CUDA(cudaEventRecord(p->ev_last_use, cs));
+  }
+  FC_CUDA(cudaEventRecord(c->ev_pack_end, cs));
+  return FC_OK;
+}
+
+// Under mu: refuses while a drain error is pending, else issues the next save ticket.
+static int next_ticket_locked(fc_ctx* c, uint64_t* ticket) {
+  if (c->drain_rc != FC_OK) return fail(c->drain_rc, "%s", c->drain_err.c_str());
+  c->ticket += 1;
+  if (ticket) *ticket = c->ticket;
+  return FC_OK;
+}
+
+// A bounded-arena save: gather and drain one window after the other on the caller's
+// thread, each window's runs under the pacing of the arena part (drain_runs).  Complete
+// on return, with its ticket drained; fc_save_timings spans the first gather to the last
+// drain.
+static int save_windowed(fc_plan* p, const std::vector<Window>& wins, uint8_t* host,
+                         cudaStream_t cs, uint64_t* ticket) {
+  fc_ctx* c = p->ctx;
+  const SliceClip clip(c, host + p->host_lo);
+  FC_CUDA(cudaStreamWaitEvent(cs, p->ev_upload, 0));
+  FC_CUDA(cudaEventRecord(c->ev_pack_start, cs));
+  for (size_t i = 0; i < wins.size(); ++i) {
+    const Window& w = wins[i];
+    int rc = launch_slice<0>(p, cs, FC_VARIANT_AUTO, w.i0, w.i1, w.abase);
+    if (rc) return rc;
+    FC_CUDA(cudaEventRecord(c->ev_pack_end, cs));
+    FC_CUDA(cudaStreamWaitEvent(c->copy_stream, c->ev_pack_end, 0));
+    if (i == 0) FC_CUDA(cudaEventRecord(c->ev_drain_start, c->copy_stream));
+    const cudaError_t e =
+        drain_runs(c, host, run_segs(p, w.base, w.end, w.abase), clip, &c->n_memcpys);
+    if (e != cudaSuccess)
+      return fail(FC_ECUDA, "bounded-arena drain: %s%s", cudaGetErrorString(e));
+    // the next gather overwrites the window: it must wait for this drain
+    FC_CUDA(cudaEventRecord(c->ev_drain_end, c->copy_stream));
+    FC_CUDA(cudaStreamWaitEvent(cs, c->ev_drain_end, 0));
+  }
+  FC_CUDA(cudaEventRecord(c->ev_pack_end, cs));
+  FC_CUDA(cudaEventRecord(p->ev_last_use, cs));
+  FC_CUDA(cudaEventRecord(c->ev_drain_end, c->copy_stream));
+  FC_CUDA(cudaEventSynchronize(c->ev_drain_end));
+  FC_CUDA(cudaEventSynchronize(c->ev_pack_end));
+  std::lock_guard<std::mutex> lk(c->mu);
+  int rc = next_ticket_locked(c, ticket);
+  if (rc) return rc;
+  c->stat_ticket = c->ticket;
+  c->stat_bytes = p->payload;
+  c->stat_delta = 0;
+  c->drained_ticket = c->ticket;
+  return FC_OK;
+}
+
+// Issues the save's ticket and hands its drain to the pump, with the records the form sets.
+static int save_enqueue(fc_plan* p, const SaveForm& f, uint8_t* host, fc_ctx::DrainJob& job,
+                        uint64_t* ticket) {
+  fc_ctx* c = p->ctx;
+  {
+    std::lock_guard<std::mutex> lk(c->mu);
+    int rc = next_ticket_locked(c, ticket);
+    if (rc) return rc;
+    if (!c->pump.joinable()) c->pump = std::thread(pump_main, c);
+    job.ticket = c->ticket;
+    if (f.hold) c->held_ticket = c->ticket;
+    if (f.in_place) c->direct_ticket = c->ticket;
+    c->jobs.push_back(std::move(job));
+    c->save_inflight = true;
+    if (f.incremental) {
+      c->base_plan = p;
+      c->base_host = host;
+      c->base_ticket = c->ticket;
+    }
+    if (!f.in_place) image_expect_locked(c, p, host, c->ticket);
+  }
+  c->cv.notify_all();
+  return FC_OK;
+}
+
+static int save(fc_plan* p, void* host_base, void* compute_stream, uint64_t* ticket,
+                const SaveForm& f) {
+  if (!p || (!host_base && p->payload)) return fail(FC_EINVAL, "%s: null argument%s", f.who);
+  fc_ctx* c = p->ctx;
+  FC_GUARD(c);
+  SaveScope s;
+  int rc = save_begin(p, f, &s);
+  if (rc) return rc;
+  uint8_t* host = static_cast<uint8_t*>(host_base);
+  cudaStream_t cs = (cudaStream_t)compute_stream;
+  bool compare;
+  {
+    // the arena changes now; an incremental save's baseline is valid again once it drained
+    std::lock_guard<std::mutex> lk(c->mu);
+    compare = f.incremental && c->base_valid && c->base_plan == p && c->base_host == host;
+    delta_forget_locked(c);
+  }
+  if (!s.wins.empty()) return save_windowed(p, s.wins, host, cs, ticket);
+  rc = save_gather(p, cs, s, compare);
+  if (rc) return rc;
+  fc_ctx::DrainJob job;
+  job.host = host;
+  job.direct = f.in_place;
+  for (const FcSpan& sp : p->spans)
+    if (sp.off < f.cut) job.spans.push_back({(uint8_t*)(uintptr_t)sp.tptr, sp.off, sp.len});
+  if (compare) {
+    job.delta = p->dmap;
+    job.seq = c->delta_seq;
+  } else {
+    job.runs = run_segs(p, f.cut, ~0ull, s.abase);
+  }
+  job.staged_threads =
+      p->runs.empty() ? 0 : staged_threads_for(c, host + p->host_lo, p->host_hi - p->host_lo);
+  return save_enqueue(p, f, host, job, ticket);
+}
+
+//                                                        who, cut, in_place, incremental, hold
 extern "C" int fc_save_async(fc_plan* p, void* host_base, void* compute_stream, uint64_t* ticket) {
-  return save_async_impl(p, host_base, compute_stream, ticket, false);
+  return save(p, host_base, compute_stream, ticket, {"fc_save_async", 0, false, false, false});
 }
 
 extern "C" int fc_save_async_held(fc_plan* p, void* host_base, void* compute_stream,
                                   uint64_t* ticket) {
-  return save_async_impl(p, host_base, compute_stream, ticket, true);
+  return save(p, host_base, compute_stream, ticket, {"fc_save_async", 0, false, false, true});
+}
+
+extern "C" int fc_save_hybrid_async(fc_plan* p, void* host_base, void* compute_stream,
+                                    uint64_t cut, int hold, uint64_t* ticket) {
+  return save(p, host_base, compute_stream, ticket,
+              {"fc_save_hybrid_async", cut, true, false, hold != 0});
+}
+
+extern "C" int fc_save_direct_async(fc_plan* p, void* host_base, void* compute_stream, int hold,
+                                    uint64_t* ticket) {
+  return save(p, host_base, compute_stream, ticket,
+              {"fc_save_hybrid_async", ~0ull, true, false, hold != 0});
+}
+
+extern "C" int fc_save_delta_async(fc_plan* p, void* host_base, void* compute_stream, int hold,
+                                   uint64_t* ticket) {
+  return save(p, host_base, compute_stream, ticket,
+              {"fc_save_delta_async", 0, false, true, hold != 0});
 }
 
 extern "C" int fc_save_release(fc_ctx* c, uint64_t ticket) {
@@ -1859,283 +2104,7 @@ extern "C" int fc_save_cancel(fc_ctx* c, uint64_t ticket) {
   return FC_OK;
 }
 
-static int save_async_impl(fc_plan* p, void* host_base, void* compute_stream, uint64_t* ticket,
-                           bool hold) {
-  if (!p || (!host_base && p->payload)) return fail(FC_EINVAL, "fc_save_async: null argument%s%s");
-  fc_ctx* c = p->ctx;
-  FC_GUARD(c);
-  int rc = refresh_inflight(c);
-  if (rc) return rc;
-  if (c->save_inflight || c->restore_inflight)
-    return fail(FC_EBUSY, "fc_save_async: previous save/restore still draining%s%s");
-  delta_forget(c);
-  cudaStream_t cs = (cudaStream_t)compute_stream;
-  if (p->arena_end > c->arena_bytes) {
-    if (c->arena_bytes < (8ull << 20) || !p->identity)
-      return fail(FC_EINVAL, "arena smaller than the plan: call fc_arena_reserve first%s%s");
-    rc = save_windowed(p, static_cast<uint8_t*>(host_base), cs);
-    if (rc) return rc;
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->ticket += 1;
-    c->stat_ticket = c->ticket;
-    c->stat_bytes = p->payload;
-    c->stat_delta = 0;
-    c->drained_ticket = c->ticket;  // already complete
-    if (ticket) *ticket = c->ticket;
-    return FC_OK;
-  }
-  {
-    // a sticky drain error must surface BEFORE the arena is overwritten
-    std::lock_guard<std::mutex> lk(c->mu);
-    if (c->drain_rc != FC_OK) return fail(c->drain_rc, "%s", c->drain_err.c_str());
-  }
-  FC_CUDA(cudaEventRecord(c->ev_pack_start, cs));
-  rc = launch_copy<0>(p, cs, FC_VARIANT_AUTO);
-  if (rc) return rc;
-  FC_CUDA(cudaEventRecord(c->ev_pack_end, cs));
-  const int staged =
-      p->runs.empty() ? 0
-                      : staged_threads_for(c, static_cast<uint8_t*>(host_base) + p->host_lo,
-                                           p->host_hi - p->host_lo);
-  // hand the drain to the pump thread (paced submission, see kDrainPiece)
-  {
-    std::lock_guard<std::mutex> lk(c->mu);
-    if (c->drain_rc != FC_OK) return fail(c->drain_rc, "%s", c->drain_err.c_str());
-    if (!c->pump.joinable()) c->pump = std::thread(pump_main, c);
-    c->ticket += 1;
-    fc_ctx::DrainJob job;
-    job.staged_threads = staged;
-    job.host = static_cast<uint8_t*>(host_base);
-    job.runs = p->runs;
-    job.ticket = c->ticket;
-    if (hold) c->held_ticket = c->ticket;
-    c->jobs.push_back(std::move(job));
-    c->save_inflight = true;
-    image_expect_locked(c, p, static_cast<uint8_t*>(host_base), c->ticket);
-    if (ticket) *ticket = c->ticket;
-  }
-  c->cv.notify_all();
-  return FC_OK;
-}
-
-// In-place part below `cut` (DMA from the tensors, drained first), snapshot part at
-// and above it: the same bulk/shift/resid kernels as a full save, over the table
-// slices from the cut on, into the arena whose byte 0 stands for segment offset
-// `cut` rounded down to 128 B.
-static int save_hybrid_impl(fc_plan* p, void* host_base, void* compute_stream, uint64_t cut,
-                            int hold, uint64_t* ticket) {
-  if (!p || (!host_base && p->payload))
-    return fail(FC_EINVAL, "fc_save_hybrid_async: null argument%s%s");
-  fc_ctx* c = p->ctx;
-  FC_GUARD(c);
-  int rc = refresh_inflight(c);
-  if (rc) return rc;
-  if (c->save_inflight || c->restore_inflight)
-    return fail(FC_EBUSY, "fc_save_hybrid_async: previous save/restore still draining%s%s");
-  delta_forget(c);
-  if (!p->identity && cut != ~0ull)
-    return fail(FC_EINVAL, "fc_save_hybrid_async: needs a plan whose arena is an image of "
-                           "the segment%s%s");
-  cudaStream_t cs = (cudaStream_t)compute_stream;
-  const std::vector<FcItem>& it = p->h_all;
-  uint32_t n = (uint32_t)it.size();
-  uint32_t i0 = (uint32_t)(std::lower_bound(it.begin(), it.end(), cut,
-                                            [](const FcItem& a, uint64_t v) { return a.aoff < v; }) -
-                           it.begin());
-  if (i0 > 0 && it[i0 - 1].aoff + it[i0 - 1].nbytes > cut)
-    return fail(FC_EINVAL, "fc_save_hybrid_async: cut is not a tensor boundary%s%s");
-  const uint64_t abase = arena_base_for(std::min(cut, p->arena_end));
-  if (i0 < n && p->arena_end - abase > c->arena_bytes)
-    return fail(FC_EINVAL, "fc_save_hybrid_async: arena smaller than the snapshot part%s%s");
-  {
-    // a sticky drain error must surface BEFORE the arena is overwritten
-    std::lock_guard<std::mutex> lk(c->mu);
-    if (c->drain_rc != FC_OK) return fail(c->drain_rc, "%s", c->drain_err.c_str());
-  }
-  // with no kernel the pair of events still orders the drain after everything
-  // already queued on the training stream (the optimizer step that produced the values)
-  FC_CUDA(cudaEventRecord(c->ev_pack_start, cs));
-  if (i0 < n) {
-    FC_CUDA(cudaStreamWaitEvent(cs, p->ev_upload, 0));
-    rc = launch_slice<0>(p, cs, FC_VARIANT_AUTO, i0, n, abase);
-    if (rc) return rc;
-    FC_CUDA(cudaEventRecord(p->ev_last_use, cs));
-  }
-  FC_CUDA(cudaEventRecord(c->ev_pack_end, cs));
-  const int staged =
-      p->spans.empty() ? 0
-                       : staged_threads_for(c, static_cast<uint8_t*>(host_base) + p->host_lo,
-                                            p->host_hi - p->host_lo);
-  {
-    std::lock_guard<std::mutex> lk(c->mu);
-    if (c->drain_rc != FC_OK) return fail(c->drain_rc, "%s", c->drain_err.c_str());
-    if (!c->pump.joinable()) c->pump = std::thread(pump_main, c);
-    c->ticket += 1;
-    fc_ctx::DrainJob job;
-    job.staged_threads = staged;
-    job.host = static_cast<uint8_t*>(host_base);
-    for (const FcSpan& sp : p->spans)
-      if (sp.off < cut) job.spans.push_back(sp);
-    for (const FcRun& r : p->runs) {
-      uint64_t a = std::max(r.off, cut), b = r.off + r.len;
-      if (b > a) job.runs.push_back({a, b - a, a});
-    }
-    job.direct = true;
-    job.arena_base = abase;
-    job.ticket = c->ticket;
-    if (hold) c->held_ticket = c->ticket;
-    c->direct_ticket = c->ticket;
-    c->jobs.push_back(std::move(job));
-    c->save_inflight = true;
-    if (ticket) *ticket = c->ticket;
-  }
-  c->cv.notify_all();
-  return FC_OK;
-}
-
-extern "C" int fc_save_hybrid_async(fc_plan* p, void* host_base, void* compute_stream,
-                                    uint64_t cut, int hold, uint64_t* ticket) {
-  return save_hybrid_impl(p, host_base, compute_stream, cut, hold, ticket);
-}
-
-extern "C" int fc_save_direct_async(fc_plan* p, void* host_base, void* compute_stream, int hold,
-                                    uint64_t* ticket) {
-  return save_hybrid_impl(p, host_base, compute_stream, ~0ull, hold, ticket);
-}
-
-// ---- incremental save --------------------------------------------------------------
-
 static int check_ticket(fc_ctx* c, uint64_t ticket, const char* who);
-
-static int launch_delta_lsu(fc_ctx* c, const FcItem* items, uint32_t n, cudaStream_t s,
-                            uint32_t seq) {
-  if (n == 0) return FC_OK;
-  uint32_t grid = std::min<uint32_t>(n, (uint32_t)(c->sm_count * c->lsu_ctas_per_sm));
-  fc_delta_lsu<<<grid, kLsuThreads, 0, s>>>(items, n, c->arena, c->dirty, seq);
-  FC_CUDA(cudaGetLastError());
-  c->n_kernels += 1;
-  return FC_OK;
-}
-
-// The ring takes the copy ring's shared memory (fc_set_launch): a stage holds a source
-// and an old tile of half the copy tile each (default 2 stages x 2 x 48 KiB).
-static int launch_delta_tma(fc_ctx* c, const FcItem* items, uint32_t n, cudaStream_t s,
-                            uint32_t seq) {
-  if (n == 0) return FC_OK;
-  const uint32_t tile = std::max<uint32_t>(128u, ((uint32_t)c->tma_tile / 2u) & ~127u);
-  const uint32_t stages = (uint32_t)c->tma_stages;
-  const size_t smem = delta_smem_bytes(tile, stages);
-  FC_CUDA(cudaFuncSetAttribute(fc_delta_tma, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)smem));
-  uint32_t grid = std::min<uint32_t>(n, (uint32_t)(c->sm_count * c->tma_ctas_per_sm));
-  fc_delta_tma<<<grid, kDeltaThreads, smem, s>>>(items, n, c->arena, c->dirty, seq, tile, stages);
-  FC_CUDA(cudaGetLastError());
-  c->n_kernels += 1;
-  return FC_OK;
-}
-
-// Gather-compare over the whole plan: bulk bodies through the TMA ring, shifted ranges
-// and residues through the LSU kernel (FC_VARIANT_LSU: every item through the LSU kernel).
-static int launch_delta(fc_plan* p, cudaStream_t s, uint32_t seq) {
-  fc_ctx* c = p->ctx;
-  FC_CUDA(cudaStreamWaitEvent(s, p->ev_upload, 0));
-  int rc;
-  if (c->variant == FC_VARIANT_TMA) {
-    rc = launch_delta_tma(c, p->bulk.dev, p->bulk.n, s, seq);
-    if (!rc) rc = launch_delta_lsu(c, p->shift.dev, p->shift.n, s, seq);
-    if (!rc) rc = launch_delta_lsu(c, p->resid.dev, p->resid.n, s, seq);
-  } else {
-    rc = launch_delta_lsu(c, p->all.dev, p->all.n, s, seq);
-  }
-  if (rc) return rc;
-  FC_CUDA(cudaEventRecord(p->ev_last_use, s));
-  return FC_OK;
-}
-
-extern "C" int fc_save_delta_async(fc_plan* p, void* host_base, void* compute_stream, int hold,
-                                   uint64_t* ticket) {
-  if (!p || (!host_base && p->payload))
-    return fail(FC_EINVAL, "fc_save_delta_async: null argument%s%s");
-  fc_ctx* c = p->ctx;
-  FC_GUARD(c);
-  int rc = refresh_inflight(c);
-  if (rc) return rc;
-  if (c->save_inflight || c->restore_inflight)
-    return fail(FC_EBUSY, "fc_save_delta_async: previous save/restore still draining%s%s");
-  if (p->arena_end > c->arena_bytes)
-    return fail(FC_EINVAL, "fc_save_delta_async: the arena must hold the whole plan (no "
-                           "incremental bounded-arena save)%s%s");
-  uint8_t* host = static_cast<uint8_t*>(host_base);
-  bool delta;
-  {
-    std::lock_guard<std::mutex> lk(c->mu);
-    // a sticky drain error must surface BEFORE the arena is overwritten
-    if (c->drain_rc != FC_OK) return fail(c->drain_rc, "%s", c->drain_err.c_str());
-    delta = c->base_valid && c->base_plan == p && c->base_host == host;
-    delta_forget_locked(c);  // the arena changes now; valid again once this save drained
-  }
-  cudaStream_t cs = (cudaStream_t)compute_stream;
-  const uint32_t n_all = p->all.n;
-  bool reset = false;
-  if (delta && n_all > c->dirty_cap) {
-    const uint32_t cap = (uint32_t)std::min<uint64_t>(0xFFFFFFF0ull, n_all + n_all / 4 + 16);
-    uint32_t* nd = nullptr;
-    uint32_t* np = nullptr;
-    cudaError_t e = cudaMalloc(&nd, (size_t)cap * sizeof(uint32_t));
-    if (e == cudaSuccess) e = cudaHostAlloc(&np, (size_t)cap * sizeof(uint32_t), cudaHostAllocDefault);
-    if (e != cudaSuccess) {
-      (void)cudaGetLastError();
-      if (nd) c->dead_dev.push_back(nd);
-      return fail(FC_ENOMEM, "dirty marks alloc: %s", cudaGetErrorString(e));
-    }
-    if (c->dirty) c->dead_dev.push_back(c->dirty);  // no save is in flight: nothing reads them
-    if (c->dirty_pinned) c->dead_pinned.push_back(c->dirty_pinned);
-    c->dirty = nd;
-    c->dirty_pinned = np;
-    c->dirty_cap = cap;
-    reset = true;
-  }
-  if (delta) {
-    // marks are sequence numbers: cleared only for a fresh array or when seq wraps
-    if (++c->delta_seq == 0) reset = true;
-    if (reset) {
-      FC_CUDA(cudaMemsetAsync(c->dirty, 0, (size_t)c->dirty_cap * sizeof(uint32_t), cs));
-      c->delta_seq = 1;
-    }
-  }
-  FC_CUDA(cudaEventRecord(c->ev_pack_start, cs));
-  rc = delta ? launch_delta(p, cs, c->delta_seq) : launch_copy<0>(p, cs, FC_VARIANT_AUTO);
-  if (rc) return rc;
-  FC_CUDA(cudaEventRecord(c->ev_pack_end, cs));
-  const int staged =
-      p->runs.empty() ? 0 : staged_threads_for(c, host + p->host_lo, p->host_hi - p->host_lo);
-  {
-    std::lock_guard<std::mutex> lk(c->mu);
-    if (c->drain_rc != FC_OK) return fail(c->drain_rc, "%s", c->drain_err.c_str());
-    if (!c->pump.joinable()) c->pump = std::thread(pump_main, c);
-    c->ticket += 1;
-    fc_ctx::DrainJob job;
-    job.staged_threads = staged;
-    job.host = host;
-    if (delta) {
-      job.delta = p->dmap;
-      job.seq = c->delta_seq;
-    } else {
-      job.runs = p->runs;
-    }
-    job.ticket = c->ticket;
-    if (hold) c->held_ticket = c->ticket;
-    c->jobs.push_back(std::move(job));
-    c->save_inflight = true;
-    c->base_plan = p;
-    c->base_host = host;
-    c->base_ticket = c->ticket;
-    image_expect_locked(c, p, host, c->ticket);
-    if (ticket) *ticket = c->ticket;
-  }
-  c->cv.notify_all();
-  return FC_OK;
-}
 
 extern "C" int fc_save_delta_stats(fc_ctx* c, uint64_t ticket, uint64_t* drained_bytes,
                                    int* delta) {
@@ -2163,7 +2132,7 @@ extern "C" int fc_restore_direct_async(fc_plan* p, const void* host_base, void* 
   int rc = restore_begin(c, "fc_restore_direct_async: context busy");
   if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream;
-  std::vector<FillSeg> segs;
+  std::vector<Seg> segs;
   for (const FcSpan& sp : p->spans) segs.push_back({(uint8_t*)(uintptr_t)sp.tptr, sp.off, sp.len});
   const FillSource src{static_cast<const uint8_t*>(host_base), nullptr, "staged restore"};
   rc = restore_fill_gated(c, s, segs, src);

@@ -83,7 +83,9 @@ int fc_arena_info(fc_ctx* ctx, void** dev_ptr, uint64_t* bytes);
  * (gather window -> DMA -> next window).  The tensors must stay unchanged until
  * the last window is gathered, so in this mode fc_save_async returns only when
  * the whole checkpoint is in host memory (the reference's blocking behaviour,
- * at PCIe speed).  Use when the state does not fit in HBM a second time. */
+ * at PCIe speed).  Each window drains under the context's drain pacing
+ * (fc_set_drain, fc_set_drain_mode).  Use when the state does not fit in HBM a
+ * second time. */
 int fc_set_arena_limit(fc_ctx* ctx, uint64_t bytes);
 
 /* Pin (cudaHostRegister) a host range the CALLER mapped — the POSIX shm
@@ -189,10 +191,10 @@ int fc_set_shift_launch(fc_ctx* ctx, int ctas_per_sm, int in_stages, int tile_by
 /* Enqueue the pack kernel on `compute_stream` (the ONLY work the training
  * stream waits for), then on the context's copy stream — gated by an event,
  * never by a host sync — DMA every arena run to host_base+offset in
- * <= drain_chunk pieces.  host_base should be fc_host_register()-ed; if it is
- * not the copies still work but are staged by the driver.  One save may be in
- * flight per context (FC_EBUSY otherwise).  Replaces _traverse_copy_to_shm
- * (ckpt_saver.py:198-218). */
+ * <= drain_piece pieces (fc_set_drain).  host_base should be
+ * fc_host_register()-ed; if it is not, the copies go through the context's
+ * pinned bounce slots (fc_set_stage).  One save may be in flight per context
+ * (FC_EBUSY otherwise).  Replaces _traverse_copy_to_shm (ckpt_saver.py:198-218). */
 int fc_save_async(fc_plan* plan, void* host_base, void* compute_stream,
                   uint64_t* ticket);
 /* Same, but the drain does not start until fc_save_release(ticket): lets the
@@ -277,7 +279,8 @@ int fc_save_timings(fc_ctx* ctx, uint64_t ticket, float* pack_ms, float* drain_m
  * then waits at most one piece, ~0.3 ms; 32 MiB pieces: +1.8 % throughput, +2 ms of
  * exposed stall per checkpoint).  0 keeps the current value. */
 int fc_set_drain(fc_ctx* ctx, uint64_t piece_bytes, int depth);
-/* How the pump keeps "one piece in flight":
+/* How the pump (and the bounded-arena save, window by window) keeps "one piece in
+ * flight":
  *   FC_DRAIN_HOST_PACED  the host submits piece k+1 after piece k completed (one host
  *                        round trip between two pieces; a spinning wait hides most of it);
  *   FC_DRAIN_PINGPONG    pieces alternate between two copy streams, piece k waiting on

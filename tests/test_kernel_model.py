@@ -759,6 +759,188 @@ def test_every_restore_source_writes_exactly_the_target_bytes(cuda_device, tmp_p
                 os.close(fd)
 
 
+def _window_dma_counts(items, run_list, arena_bytes, piece):
+    """DMA copies of each window of a bounded-arena save: a window takes the items from
+    the first one left on while they end within arena_bytes of its start rounded down to
+    128 B, and drains the runs clipped to the bytes it covers."""
+    counts, i = [], 0
+    while i < len(items):
+        base = end = items[i].aoff
+        abase, j = base & ~127, i
+        while j < len(items) and items[j].aoff + items[j].n - abase <= arena_bytes:
+            end = max(end, items[j].aoff + items[j].n)
+            j += 1
+        assert j > i
+        counts.append(sum(-(-(min(end, r.aoff + r.n) - max(base, r.aoff)) // piece)
+                          for r in run_list if max(base, r.aoff) < min(end, r.aoff + r.n)))
+        i = j
+    return counts
+
+
+def _save_forms(w, addr, seg, model, pinned, bounded, rng):
+    """Every save form of plan P into the host range at `addr` (its bytes `seg`, their
+    model `model`), each from a canary segment except the incremental save, which
+    follows the full one.  Checks every host, arena and source byte after each form,
+    and the DMA copies where the host range is pinned."""
+    ctx, p, stream = w.ctx, w.plans["P"], torch.cuda.current_stream()
+    plan, src = p["plan"], w.lay.src
+    ranges = [r for r in p["ranges"] if r.n]
+
+    def fresh():
+        seg[:] = model[:] = pattern(model.size)
+
+    def saved(rs=ranges):
+        for r in rs:
+            model[r.hoff:r.hoff + r.n] = src.read(r.tptr, r.n)
+
+    def check(form, copies, expected):
+        torch.cuda.synchronize()
+        if pinned:
+            assert copies == expected, f"{form}: {copies} DMA copies, the model says {expected}"
+        bad = np.flatnonzero(seg != model)
+        assert bad.size == 0, f"{form}: segment differs at {bad[:8]}"
+        w.check(form)
+
+    def run(form, call):
+        _, m0 = ctx.launch_count()
+        call()
+        return ctx.launch_count()[1] - m0
+
+    if bounded:
+        fresh()
+        copies = run("bounded", lambda: ctx.save_wait(plan.save_async(addr, stream)))
+        saved()
+        counts = _window_dma_counts(p["items"], p["runs"], ctx.arena_info()[1], w.piece)
+        assert len(counts) > 1
+        check("bounded save", copies, sum(counts))
+        return
+
+    fresh()
+    copies = run("save", lambda: ctx.save_wait(plan.save_async(addr, stream)))
+    w.arena = w._gathered("P")
+    saved()
+    check("save", copies, pm.dma_count(p["runs"], w.piece))
+
+    for release in (True, False):
+        fresh()
+
+        def held():
+            ticket = plan.save_async(addr, stream, hold=True)
+            torch.cuda.synchronize()
+            if release:
+                ctx.save_release(ticket)
+            else:
+                assert ctx.save_cancel(ticket)
+            ctx.save_wait(ticket)
+
+        copies = run("held", held)
+        w.arena = w._gathered("P")
+        if release:
+            saved()
+        check(f"held save, release={release}", copies,
+              pm.dma_count(p["runs"], w.piece) if release else 0)
+
+    fresh()
+    copies = run("direct", lambda: ctx.save_wait(plan.save_direct_async(addr, stream)))
+    saved()
+    check("in-place save", copies, pm.dma_count(ranges, w.piece))
+
+    starts = sorted(r.aoff for r in ranges)
+    for cut in (starts[len(starts) // 3], starts[2 * len(starts) // 3]):
+        fresh()
+        copies = run("hybrid",
+                     lambda: ctx.save_wait(plan.save_hybrid_async(addr, cut, stream)))
+        abase = cut & ~127
+        for r in ranges:
+            if r.aoff >= cut:
+                w.arena[r.aoff - abase:r.aoff - abase + r.n] = src.read(r.tptr, r.n)
+        saved()
+        head = [r for r in ranges if r.hoff < cut]
+        tail = pm.runs([r for r in ranges if r.aoff >= cut])
+        check(f"hybrid save at {cut}", copies,
+              pm.dma_count(head, w.piece) + pm.dma_count(tail, w.piece))
+
+    fresh()
+    ticket = [0]
+
+    def delta():
+        ticket[0] = plan.save_delta_async(addr, stream)
+        ctx.save_wait(ticket[0])
+
+    copies = run("delta", delta)
+    w.arena = w._gathered("P")
+    saved()
+    assert ctx.save_delta_stats(ticket[0]) == (False, sum(r.n for r in ranges))
+    check("full incremental save", copies, pm.dma_count(p["runs"], w.piece))
+    for kind in ("leaf", "span", "byte"):
+        _change(w, rng, kind)
+    new = w._gathered("P")
+    d = pm.dirty(p["items"], w.arena, new, w.arena_lo)
+    assert d
+    copies = run("delta", delta)
+    w.arena = new
+    saved()
+    assert ctx.save_delta_stats(ticket[0]) == (True, pm.drained_bytes(d))
+    check("incremental save", copies, pm.dma_count(pm.runs(d), w.piece))
+
+
+@gpu
+@pytest.mark.parametrize("mode", [native.DRAIN_HOST_PACED, native.DRAIN_PINGPONG],
+                         ids=["host_paced", "pingpong"])
+@pytest.mark.parametrize("variant", VARIANTS, ids=["lsu", "tma"])
+@pytest.mark.parametrize("layout", ["state_dict", "mixed"])
+def test_every_save_form_writes_exactly_the_segment_bytes(cuda_device, layout, variant, mode):
+    """Every save form (full, held and released, held and cancelled, in place, hybrid at
+    two cuts, incremental full and then incremental, and through an 8 MiB arena) into
+    the pinned segment, a plain mapping (bounce slots) and a mapping registered slice by
+    slice, in 64-KiB drain pieces."""
+    rng = np.random.default_rng(11 + variant * 2 + mode)
+    lay = (state_dict_layout(10) if layout == "state_dict"
+           else mixed_layout(10, _tiles("default"), DEFAULT_CHUNK))
+    piece = 64 << 10
+    for bounded in (False, True):
+        ctx = _context("default", variant, 8 << 20 if bounded else 0)
+        ctx.set_stage(3, 1 << 20)
+        ctx.set_drain_mode(mode)
+        ctx.set_drain(piece)
+        with _world(ctx, lay, 0, variant, piece=piece, bounded=bounded) as w:
+            assert (ctx.arena_info()[1] < lay.arena_end) == bounded
+            a = w.host_t["A"]
+            _save_forms(w, a.data_ptr(), a.numpy(), w.host["A"], True, bounded, rng)
+            model = pattern(w.host["A"].size)
+            with _plain_mapping(model) as addr:
+                seg = np.ctypeslib.as_array((ctypes.c_uint8 * model.size).from_address(addr))
+                _save_forms(w, addr, seg, model, False, bounded, rng)
+                ctx.host_register_background(addr, model.size, slice_bytes=2 << 20)
+                deadline = time.time() + 60
+                while not ctx.host_ready(addr):
+                    assert time.time() < deadline
+                    time.sleep(0.01)
+                _save_forms(w, addr, seg, model, False, bounded, rng)
+                ctx.host_unregister(addr)
+                del seg
+
+
+@gpu
+def test_a_refused_save_keeps_the_baseline_and_the_image(cuda_device):
+    """A save refused for its arguments (a hybrid cut inside a tensor) touches neither
+    the incremental baseline nor the arena image: the next incremental save compares
+    and drains nothing."""
+    ctx = _context("default", native.VARIANT_TMA)
+    with _world(ctx, _small_layout(5, "default"), 4096, native.VARIANT_TMA) as w:
+        w.delta()
+        w.check("full incremental save")
+        p, addr = w.plans["P"], w.host_t["A"].data_ptr()
+        inside = next(r for r in p["ranges"] if r.n > 1).aoff + 1
+        for hold in (False, True):
+            with pytest.raises(native.NativeError) as e:
+                p["plan"].save_hybrid_async(addr, inside, torch.cuda.current_stream(), hold)
+            assert e.value.code == native.FC_EINVAL
+        assert p["plan"].image_covers(addr)
+        w.delta()  # asserts (incremental, 0 bytes drained)
+        w.check("incremental save after the refusals")
+
+
 # --------------------------------------------------------- exact incremental accounting --
 
 OPS = ("pack", "unpack", "arena_fill", "save", "save_direct", "save_hybrid", "restore",
