@@ -130,6 +130,8 @@ _SIGNATURES = {
     "fc_restore_from_image_async": (ctypes.c_int, [_vp, _vp, _vp]),
     "fc_image_covers": (ctypes.c_int, [_vp, _vp]),
     "fc_restore_file_async": (ctypes.c_int, [_vp, ctypes.c_int, _vp]),
+    "fc_restore_files_async": (ctypes.c_int, [_vp, _u32, ctypes.POINTER(ctypes.c_int),
+                                              ctypes.POINTER(_u64), _vp]),
     "fc_plan_set_kinds": (ctypes.c_int, [_vp, _u32, ctypes.POINTER(ctypes.c_uint8)]),
     "fc_scan_nonfinite_async": (ctypes.c_int, [_vp, _vp]),
     "fc_scan_wait": (ctypes.c_int, [_vp, ctypes.POINTER(_u64), ctypes.POINTER(_u32), _u32]),
@@ -335,6 +337,20 @@ class Plan:
         short file or a failed read (no tensor changed)."""
         _check(load_library().fc_restore_file_async(self.handle, int(fd), _stream_ptr(stream)),
                "fc_restore_file_async")
+
+    def restore_files_async(self, fds: Sequence[int], bases: Sequence[int], stream=None):
+        """Restore from several open files in one fill and one scatter: the plan's host
+        offsets lie in their virtual concatenation, file k owning [bases[k], bases[k+1])
+        (strictly increasing).  As restore_file_async otherwise; NativeError with code
+        FC_EIO names the file index when one is short or a read fails (no tensor changed)."""
+        n = len(fds)
+        if len(bases) != n:
+            raise ValueError(f"restore_files_async: {n} files but {len(bases)} bases")
+        a_fd = (ctypes.c_int * max(n, 1))(*[int(f) for f in fds])
+        a_base = (_u64 * max(n, 1))(*[int(b) for b in bases])
+        _check(load_library().fc_restore_files_async(self.handle, n, a_fd, a_base,
+                                                     _stream_ptr(stream)),
+               "fc_restore_files_async")
 
     def image_covers(self, host_ptr: int) -> bool:
         """Whether restore_from_image_async would find an image covering this plan (no

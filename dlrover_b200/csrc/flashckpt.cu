@@ -293,33 +293,50 @@ struct StagePiece {
   uint8_t* dev;
   uint8_t* host;
   uint64_t len;
-  uint64_t foff;  // file offset when the source is a file (StageFile), else unused
+  uint64_t foff;  // offset in the files' virtual concatenation (StageFile), else unused
 };
 
-// Cuts every segment into slot-sized pieces.  host == nullptr: the segments' offsets are
+// Cuts every segment into slot-sized pieces, and at every offset of `cuts` (sorted; the
+// file boundaries of a multi-file source).  host == nullptr: the segments' offsets are
 // file offsets.
 static std::vector<StagePiece> stage_pieces(const std::vector<Seg>& segs, uint8_t* host,
-                                            uint64_t slot) {
+                                            uint64_t slot,
+                                            const std::vector<uint64_t>* cuts = nullptr) {
   std::vector<StagePiece> out;
   for (const Seg& g : segs)
-    for (uint64_t o = 0; o < g.len; o += slot)
-      out.push_back({g.dev + o, host ? host + g.off + o : nullptr,
-                     std::min<uint64_t>(slot, g.len - o), g.off + o});
+    for (uint64_t o = 0, len = 0; o < g.len; o += len) {
+      len = std::min<uint64_t>(slot, g.len - o);
+      if (cuts) {
+        auto it = std::upper_bound(cuts->begin(), cuts->end(), g.off + o);
+        if (it != cuts->end()) len = std::min<uint64_t>(len, *it - (g.off + o));
+      }
+      out.push_back({g.dev + o, host ? host + g.off + o : nullptr, len, g.off + o});
+    }
   return out;
 }
 
-// A file as the source of a staged fill (fc_restore_file_async): the workers pread each
-// piece's file bytes into their slot instead of a memcpy from a host mapping.  The first
-// short read or I/O error stops every worker and is remembered here.
+// Files as the source of a staged fill (fc_restore_files_async): the workers pread each
+// piece's bytes into their slot instead of a memcpy from a host mapping.  The pieces'
+// offsets lie in the virtual concatenation of the files: file k owns [bases[k],
+// bases[k+1]), and no piece crosses a base.  The first short read or I/O error stops every
+// worker and is remembered here.
 struct StageFile {
-  int fd = -1;
+  std::vector<int> fds;
+  std::vector<uint64_t> bases;
   std::atomic<bool> failed{false};
   std::mutex mu;
-  uint64_t bad_off = 0;  // file offset of the first byte that could not be read
-  int err_no = 0;        // 0: end of file (short read)
+  uint32_t bad_file = 0;  // index of the file that could not be read
+  uint64_t bad_off = 0;   // offset in that file of the first byte that could not be read
+  int err_no = 0;         // 0: end of file (short read)
+  // the file holding virtual offset `off` (bases[0] <= off)
+  uint32_t file_of(uint64_t off) const {
+    return (uint32_t)(std::upper_bound(bases.begin(), bases.end(), off) - bases.begin() - 1);
+  }
   bool read(uint8_t* dst, uint64_t len, uint64_t off) {
+    const uint32_t k = file_of(off);
+    off -= bases[k];
     for (uint64_t got = 0; got < len;) {
-      const ssize_t r = pread(fd, dst + got, len - got, (off_t)(off + got));
+      const ssize_t r = pread(fds[k], dst + got, len - got, (off_t)(off + got));
       if (r > 0) {
         got += (uint64_t)r;
         continue;
@@ -327,6 +344,7 @@ struct StageFile {
       if (r < 0 && errno == EINTR) continue;
       std::lock_guard<std::mutex> lk(mu);
       if (!failed.load()) {
+        bad_file = k;
         bad_off = off + got;
         err_no = r < 0 ? errno : 0;
         failed.store(true);
@@ -336,6 +354,14 @@ struct StageFile {
     return true;
   }
 };
+
+// Prefix of the errors about file k of an n-file restore: the one-file call names no index.
+static void file_who(char* out, size_t cap, size_t n, uint32_t k) {
+  if (n == 1)
+    snprintf(out, cap, "fc_restore_file_async");
+  else
+    snprintf(out, cap, "fc_restore_files_async: file %u", k);
+}
 
 static cudaError_t stage_worker_init(fc_ctx* c, fc_ctx::StageWorker& w) {
   cudaError_t e = cudaSuccess;
@@ -1685,13 +1711,15 @@ static int restore_fill(fc_ctx* c, const std::vector<Seg>& segs, const FillSourc
   uint8_t* host = const_cast<uint8_t*>(src.host);
   const int staged = src.file ? c->stage_threads : staged_threads_for(c, host + lo, hi - lo);
   if (staged > 0) {
-    const std::vector<StagePiece> pieces = stage_pieces(segs, src.file ? nullptr : host,
-                                                        c->stage_slot);
+    const std::vector<StagePiece> pieces = stage_pieces(
+        segs, src.file ? nullptr : host, c->stage_slot, src.file ? &src.file->bases : nullptr);
     cudaError_t e = stage_run(c, pieces, false, gate, staged, src.file);
     if (src.file && src.file->failed.load()) {
-      char at[64];
-      snprintf(at, sizeof(at), "%llu", (unsigned long long)src.file->bad_off);
-      return fail(FC_EIO, "fc_restore_file_async: read failed at file offset %s: %s", at,
+      char who[64], at[160];
+      file_who(who, sizeof(who), src.file->fds.size(), src.file->bad_file);
+      snprintf(at, sizeof(at), "%s: read failed at file offset %llu", who,
+               (unsigned long long)src.file->bad_off);
+      return fail(FC_EIO, "%s: %s", at,
                   src.file->err_no ? strerror(src.file->err_no) : "unexpected end of file");
     }
     if (e != cudaSuccess) return fail(FC_ECUDA, "%s: %s", src.what, cudaGetErrorString(e));
@@ -2382,28 +2410,65 @@ extern "C" int fc_restore_async(fc_plan* p, const void* host_base, void* stream)
 // pinned bounce slots and DMA each slot into the arena; the scatter is enqueued only once
 // every byte has arrived, so a short read or an I/O error changes no target tensor (in
 // the windowed mode: none after the first window, whose scatter has already run).
-extern "C" int fc_restore_file_async(fc_plan* p, int fd, void* stream) {
-  if (!p || fd < 0) return fail(FC_EINVAL, "fc_restore_file_async: null plan or bad fd%s%s");
+// Several files: the plan's host offsets lie in their virtual concatenation (file k owns
+// [bases[k], bases[k+1])).  One fill reads every file, then one scatter runs.
+static int restore_files(fc_plan* p, uint32_t n, const int* fds, const uint64_t* bases,
+                         void* stream) {
   fc_ctx* c = p->ctx;
   FC_GUARD(c);
-  int rc = restore_begin(c, "fc_restore_file_async: arena busy");
+  char who[64], at[160], end[64];
+  int rc = restore_begin(c, n == 1 ? "fc_restore_file_async: arena busy"
+                                   : "fc_restore_files_async: arena busy");
   if (rc) return rc;
-  struct stat st;
-  if (fstat(fd, &st) != 0) return fail(FC_EIO, "fc_restore_file_async: fstat: %s%s", strerror(errno));
-  char at[64], end[64];
-  if (!p->runs.empty() && (uint64_t)st.st_size < p->host_hi) {
-    // a truncated file: refuse before any byte moves, in every mode
-    snprintf(at, sizeof(at), "%llu", (unsigned long long)p->host_hi);
-    snprintf(end, sizeof(end), "%llu", (unsigned long long)st.st_size);
-    return fail(FC_EIO, "fc_restore_file_async: the plan reads up to file offset %s, the file ends at %s",
-                at, end);
+  StageFile file;
+  file.fds.assign(fds, fds + n);
+  file.bases.assign(bases, bases + n);
+  // the highest byte the plan reads in each file, in that file's own offsets
+  std::vector<uint64_t> need(n, 0);
+  for (const FcRun& r : p->runs) {
+    if (r.len == 0) continue;
+    if (r.hoff < bases[0])
+      return fail(FC_EINVAL, "fc_restore_files_async: the plan reads below the first file's base%s%s");
+    for (uint32_t k = file.file_of(r.hoff); k < n && bases[k] < r.hoff + r.len; ++k) {
+      const uint64_t hi = k + 1 < n ? std::min(r.hoff + r.len, bases[k + 1]) : r.hoff + r.len;
+      need[k] = std::max(need[k], hi - bases[k]);
+    }
+  }
+  // a truncated file: refuse before any byte moves, in every mode
+  for (uint32_t k = 0; k < n; ++k) {
+    file_who(who, sizeof(who), n, k);
+    struct stat st;
+    if (fstat(fds[k], &st) != 0) {
+      snprintf(at, sizeof(at), "%s: fstat", who);
+      return fail(FC_EIO, "%s: %s", at, strerror(errno));
+    }
+    if ((uint64_t)st.st_size < need[k]) {
+      snprintf(at, sizeof(at), "%s: the plan reads up to file offset %llu", who,
+               (unsigned long long)need[k]);
+      snprintf(end, sizeof(end), "%llu", (unsigned long long)st.st_size);
+      return fail(FC_EIO, "%s, the file ends at %s", at, end);
+    }
   }
   if (p->arena_end > c->arena_bytes && c->arena_bytes < (8ull << 20))
     return fail(FC_EINVAL, "arena smaller than the plan: call fc_arena_reserve first%s%s");
-  StageFile file;
-  file.fd = fd;
   const FillSource src{nullptr, &file, "file restore"};
   return restore_arena(p, (cudaStream_t)stream, &src);
+}
+
+extern "C" int fc_restore_file_async(fc_plan* p, int fd, void* stream) {
+  if (!p || fd < 0) return fail(FC_EINVAL, "fc_restore_file_async: null plan or bad fd%s%s");
+  const uint64_t base = 0;
+  return restore_files(p, 1, &fd, &base, stream);
+}
+
+extern "C" int fc_restore_files_async(fc_plan* p, uint32_t n, const int* fds,
+                                      const uint64_t* bases, void* stream) {
+  if (!p || n == 0 || !fds || !bases)
+    return fail(FC_EINVAL, "fc_restore_files_async: null plan, no files or null array%s%s");
+  for (uint32_t k = 0; k < n; ++k)
+    if (fds[k] < 0 || (k > 0 && bases[k] <= bases[k - 1]))
+      return fail(FC_EINVAL, "fc_restore_files_async: bad fd or bases not strictly increasing%s%s");
+  return restore_files(p, n, fds, bases, stream);
 }
 
 // ---- rollback from the arena image ----------------------------------------------

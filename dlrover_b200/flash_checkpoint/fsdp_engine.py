@@ -25,6 +25,7 @@ import dataclasses
 import io
 import os
 import pickle
+import time
 from dataclasses import dataclass
 from pathlib import Path
 from typing import Any, Dict, List, Optional, Tuple, Union
@@ -597,6 +598,154 @@ class FileReader(StorageReader):
         return True
 
 
+def _item_rows(md: TensorStorageMetadata, item: ReadItem, info: _StorageInfo):
+    """(file offset, nbytes) rows, in logical order, of the box a tensor item reads from
+    its stored chunk: `lengths` at `storage_offsets` of the row-major chunk at
+    `info.offset`.  None when the box has more rows than _view_rows takes."""
+    from ..shm_handler import _view_rows
+
+    shape = _chunk_shape(md, item)
+    strides, s = [], 1
+    for n in reversed(shape):
+        strides.insert(0, s)
+        s *= n
+    first = sum(int(o) * st for o, st in zip(item.storage_offsets, strides))
+    rows = _view_rows(tuple(item.lengths), strides, first, md.properties.dtype.itemsize)
+    return None if rows is None else [(info.offset + o, n) for o, n in rows]
+
+
+def _target_rows(t: torch.Tensor):
+    """(address, nbytes) rows of a dense or row-strided tensor in logical order, else None.
+    CUDA rows follow _row_ranges' minimum row size; a CPU row is one pread of any size."""
+    from ..shm_handler import _row_ranges
+
+    if t.is_contiguous():
+        return [(t.data_ptr(), t.numel() * t.element_size())]
+    rows = _row_ranges(t, 0) if t.is_cuda else _row_ranges(t, 0, min_row_bytes=1)
+    return None if rows is None else [(p, n) for p, _, n in rows]
+
+
+def _plan_reads(items, storage_data, state_dict_metadata, resolve):
+    """Split DCP read items into direct pieces and fallback items.  Returns (cuda, host,
+    slow, targets): cuda / host are (address, relative path, file offset, nbytes) pieces
+    into CUDA / CPU targets; slow are the items _load_item reads (BYTE_IO, a dtype
+    mismatch, a target that is neither dense nor row-strided, a box above the row cap);
+    targets are (item, resolved target) of the direct items, to commit once filled."""
+    from ..shm_handler import _pair_rows
+
+    cuda, host, slow, targets = [], [], [], []
+    for item in items:
+        info = storage_data[item.storage_index]
+        md = state_dict_metadata.get(item.storage_index.fqn)
+        if item.type == LoadItemType.BYTE_IO or not isinstance(md, TensorStorageMetadata):
+            slow.append(item)
+            continue
+        target = resolve(item).detach()
+        src = _item_rows(md, item, info)
+        dst = _target_rows(target) if target.dtype == md.properties.dtype else None
+        if src is None or dst is None:
+            slow.append(item)
+            continue
+        if tuple(target.size()) != tuple(item.lengths):
+            raise ValueError(f"{item.storage_index.fqn}: the read item asks for "
+                             f"{tuple(item.lengths)}, the target is {tuple(target.size())}")
+        out = cuda if target.is_cuda else host
+        out += [(p, info.relative_path, f, n) for p, f, n in _pair_rows(src, dst) if n]
+        targets.append((item, target))
+    return cuda, host, slow, targets
+
+
+def _pread_bytes(fd: int, nbytes: int, offset: int) -> bytes:
+    parts, got = [], 0
+    while got < nbytes:
+        b = os.pread(fd, nbytes - got, offset + got)
+        if not b:
+            raise OSError(f"short read at file offset {offset + got}")
+        parts.append(b)
+        got += len(b)
+    return b"".join(parts)
+
+
+class FileDmaReader(FileReader):
+    """FileReader whose tensor items skip the per-item pageable copy: every CUDA item of
+    the plan is read through the library's file fill into the HBM arena and scattered by
+    the unpack kernels (fc_restore_files_async, one fill over every shard file this rank
+    reads), CPU items are pread straight into their targets.  Any sub-box that DCP's
+    resharding asks for is read as rows of its stored chunk, never the whole chunk.  The
+    bytes are those FileReader gives; everything else (BYTE_IO, dtype mismatches, targets
+    that are neither dense nor row-strided, boxes above the row cap) goes through
+    FileReader's path.  A shard file too short for any item raises ValueError before a
+    target changes.  `last_read_stats` describes the last read_data."""
+
+    def __init__(self, path: Union[str, os.PathLike]) -> None:
+        super().__init__(path)
+        self.last_read_stats: Dict[str, float] = {}
+
+    def read_data(self, plan: LoadPlan, planner: LoadPlanner) -> Future[None]:
+        from ..shm_handler import _pread_into, _restore_file_groups
+
+        t0 = time.perf_counter()
+        cuda, host, slow, targets = _plan_reads(plan.items, self.storage_data,
+                                                self.state_dict_metadata, planner.resolve_tensor)
+        # the highest byte every file must hold: direct pieces and whole fallback chunks
+        need: Dict[str, int] = {}
+        for _, path, f, n in cuda + host:
+            need[path] = max(need.get(path, 0), f + n)
+        for item in slow:
+            info = self.storage_data[item.storage_index]
+            need[info.relative_path] = max(need.get(info.relative_path, 0),
+                                           info.offset + info.length)
+        stats = {"device_bytes": 0.0, "host_bytes": 0.0, "fallback_items": len(slow),
+                 "files": len(need), "plans": 0, "read_ms": 0.0, "scatter_ms": 0.0,
+                 "wall_ms": 0.0}
+        fds: Dict[str, int] = {}
+        try:
+            for path in sorted(need):
+                fds[path] = os.open(self.path / path, os.O_RDONLY)
+                size = os.fstat(fds[path]).st_size
+                if size < need[path]:  # refuse before any target changes
+                    raise ValueError(f"{self.path / path}: the read items need bytes up to "
+                                     f"file offset {need[path]}, the file ends at {size}")
+            with torch.no_grad():
+                if cuda:
+                    # the files' virtual concatenation: file k starts where file k-1 ends
+                    paths = sorted({p for _, p, _, _ in cuda})
+                    bases, b = {}, 0
+                    for path in paths:
+                        bases[path] = b
+                        b += need[path]
+                    ranges = sorted(((a, bases[p] + f, n) for a, p, f, n in cuda),
+                                    key=lambda r: r[1])
+                    dev = next(t for _, t in targets if t.is_cuda).device
+                    stats["plans"] = _restore_file_groups(
+                        ranges, dev.index if dev.index is not None else torch.cuda.current_device(),
+                        None, lambda pl, s: pl.restore_files_async(
+                            [fds[p] for p in paths], [bases[p] for p in paths], s), stats)
+                t1 = time.perf_counter()
+                for a, path, f, n in host:
+                    _pread_into(fds[path], a, n, f)
+                stats["host_bytes"] = float(sum(n for _, _, _, n in host))
+                for item in slow:
+                    info = self.storage_data[item.storage_index]
+                    item_bytes = io.BytesIO(_pread_bytes(fds[info.relative_path],
+                                                         info.length, info.offset))
+                    md = None
+                    if item.type != LoadItemType.BYTE_IO:
+                        md = self.state_dict_metadata[item.storage_index.fqn]
+                    _load_item(item, item_bytes, planner, md)
+                stats["read_ms"] += (time.perf_counter() - t1) * 1e3
+            for item, target in targets:
+                planner.commit_tensor(item, target)
+        finally:
+            for fd in fds.values():
+                os.close(fd)
+        stats["wall_ms"] = (time.perf_counter() - t0) * 1e3
+        self.last_read_stats = stats
+        fut: Future = Future()
+        fut.set_result(None)
+        return fut
+
+
 def _save_planner():
     """torch's DefaultSavePlanner, minus one of its two full traversals of the state dict
     when there is nothing for it to do: `_flatten_sharded_tensors` only rewrites nested
@@ -647,6 +796,21 @@ class FsdpCheckpointEngine(CheckpointEngine):
 
     def get_saving_ranks(self):
         return None  # every rank holds a shard
+
+    # Restore from storage through the library (opt-in; also DLROVER_B200_STORAGE_DMA=1):
+    # when load() has to read the shard files, it returns a FileDmaReader instead of a
+    # FileReader.  Same bytes; the shared-memory reader is not affected.
+    _storage_dma: Optional[bool] = None
+
+    @property
+    def storage_dma(self) -> bool:
+        if self._storage_dma is None:
+            return os.getenv("DLROVER_B200_STORAGE_DMA", "0") == "1"
+        return self._storage_dma
+
+    @storage_dma.setter
+    def storage_dma(self, value: bool):
+        self._storage_dma = bool(value)
 
     # -- plan reuse ---------------------------------------------------------------------
     @staticmethod
@@ -863,7 +1027,7 @@ class FsdpCheckpointEngine(CheckpointEngine):
             resume_path = self._get_track_resume_path()
         if resume_path and os.path.exists(resume_path):
             logger.info(f"Create a storage reader with path {resume_path}.")
-            return FileReader(resume_path)
+            return FileDmaReader(resume_path) if self.storage_dma else FileReader(resume_path)
         return None
 
     def _get_track_resume_path(self):

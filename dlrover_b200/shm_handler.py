@@ -1937,6 +1937,40 @@ def _disjoint_groups(ranges):
     return groups
 
 
+def _restore_file_groups(ranges, device_index: int, stream, enqueue, stats) -> int:
+    """Restore CUDA (address, file offset, nbytes, ...) ranges, sorted by file offset,
+    through the arena of `device_index`: one mapped plan per _disjoint_groups group, whose
+    file fill enqueue(plan, stream) starts (fc_restore_file_async or
+    fc_restore_files_async).  Adds device_bytes, read_ms and scatter_ms to `stats`; returns
+    the number of plans."""
+    ctx = native.get_context(device_index)
+    if stream is None:
+        stream = torch.cuda.current_stream(device_index)
+    groups = _disjoint_groups(ranges)
+    for group in groups:
+        ptrs, arena, foffs, lens, a = [], [], [], [], 0
+        for p, f, n, *_ in group:
+            a += (p - a) % 16  # congruent to the target mod 16: the bulk kernel
+            ptrs.append(p)
+            arena.append(a)
+            foffs.append(f)
+            lens.append(n)
+            a += n
+        plan = ctx.plan(ptrs, arena, lens, host_offsets=foffs)
+        try:
+            if _DeviceStager.reserve_arena(ctx, plan.arena_end) == _DeviceStager.ARENA_NONE:
+                logger.warning(f"No room for a {plan.arena_end / 2**30:.1f} GiB restore arena "
+                               "in HBM: the file is restored window by window.")
+                ctx.arena_reserve(64 << 20)
+            got = _timed_restore(ctx, plan, lambda: enqueue(plan, stream))
+        finally:
+            plan.destroy()
+        stats["device_bytes"] += got["device_bytes"]
+        stats["read_ms"] += got["fill_ms"]
+        stats["scatter_ms"] += got["scatter_ms"]
+    return len(groups)
+
+
 def _pread_into(fd: int, address: int, nbytes: int, offset: int):
     import ctypes
 
@@ -1997,33 +2031,8 @@ def restore_file_into(path: str, target, stream=None, strict: bool = True,
                         raise ValueError(f"{name}: all CUDA leaves must live on one device; "
                                          f"got {dev} and {t.device}")
                 device_index = dev.index if dev.index is not None else torch.cuda.current_device()
-                ctx = native.get_context(device_index)
-                if stream is None:
-                    stream = torch.cuda.current_stream(device_index)
-                for group in _disjoint_groups(dev_ranges):
-                    ptrs, arena, foffs, lens, a = [], [], [], [], 0
-                    for p, f, n, _ in group:
-                        a += (p - a) % 16  # congruent to the target mod 16: the bulk kernel
-                        ptrs.append(p)
-                        arena.append(a)
-                        foffs.append(f)
-                        lens.append(n)
-                        a += n
-                    plan = ctx.plan(ptrs, arena, lens, host_offsets=foffs)
-                    try:
-                        if (_DeviceStager.reserve_arena(ctx, plan.arena_end)
-                                == _DeviceStager.ARENA_NONE):
-                            logger.warning(f"No room for a {plan.arena_end / 2**30:.1f} GiB "
-                                           "restore arena in HBM: the file is restored window "
-                                           "by window.")
-                            ctx.arena_reserve(64 << 20)
-                        got = _timed_restore(ctx, plan,
-                                             lambda: plan.restore_file_async(fd, stream))
-                    finally:
-                        plan.destroy()
-                    stats["device_bytes"] += got["device_bytes"]
-                    stats["read_ms"] += got["fill_ms"]
-                    stats["scatter_ms"] += got["scatter_ms"]
+                _restore_file_groups(dev_ranges, device_index, stream,
+                                     lambda plan, s: plan.restore_file_async(fd, s), stats)
             t1 = time.perf_counter()
             for p, f, n, _ in host:
                 _pread_into(fd, p, n, f)

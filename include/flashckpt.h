@@ -349,6 +349,23 @@ int fc_restore_timings(fc_ctx* ctx, float* fill_ms, float* scatter_ms, float* to
  * load_state_dict (reference full_ckpt_engine.py _load_from_storage). */
 int fc_restore_file_async(fc_plan* plan, int fd, void* stream);
 
+/* Restore from n open files in one fill and one scatter: the checkpoint of a resharded
+ * job, whose shards a rank reads from several files.  The plan is a mapped plan
+ * (fc_plan_create_mapped) whose host offsets lie in the virtual concatenation of the
+ * files: file k owns [bases[k], bases[k+1]) and is read at offset - bases[k]; bases is
+ * strictly increasing, so the files' offset 0 do not collide and the mapped plan's overlap
+ * rule applies as usual.  The stage workers' pieces are cut at every base, so no pread
+ * crosses a file.  An arena smaller than the plan streams it window by window, as
+ * fc_restore_file_async does.  Before anything moves, every file is checked (fstat)
+ * against the highest plan byte inside its range: FC_EIO when one is short, and
+ * fc_last_error() names the file index and offset.  A failed read returns FC_EIO too,
+ * stops every worker and enqueues no scatter.  FC_EINVAL for no files, a negative fd,
+ * bases that do not increase, or a plan byte below bases[0].  FC_EBUSY and the forgotten
+ * incremental baseline and image as in fc_restore_file_async, which is the call with
+ * n = 1 and base 0. */
+int fc_restore_files_async(fc_plan* plan, uint32_t n, const int* fds, const uint64_t* bases,
+                           void* stream);
+
 /* ---- rollback: restore from the arena image ------------------------------- */
 
 /* After a save has drained, the arena still holds a byte image of what it wrote to the
