@@ -61,6 +61,14 @@ from ..ckpt_saver import (
 from ..common import env_utils
 from ..common.constants import CheckpointConstant
 from ..common.log import default_logger as logger
+from ..shm_handler import (
+    _open_files,
+    _pair_rows,
+    _pread_into,
+    _read_pieces,
+    _target_rows,
+    _view_rows,
+)
 from .engine import (
     CheckpointEngine,
     ShardLockClaim,
@@ -602,8 +610,6 @@ def _item_rows(md: TensorStorageMetadata, item: ReadItem, info: _StorageInfo):
     """(file offset, nbytes) rows, in logical order, of the box a tensor item reads from
     its stored chunk: `lengths` at `storage_offsets` of the row-major chunk at
     `info.offset`.  None when the box has more rows than _view_rows takes."""
-    from ..shm_handler import _view_rows
-
     shape = _chunk_shape(md, item)
     strides, s = [], 1
     for n in reversed(shape):
@@ -614,25 +620,12 @@ def _item_rows(md: TensorStorageMetadata, item: ReadItem, info: _StorageInfo):
     return None if rows is None else [(info.offset + o, n) for o, n in rows]
 
 
-def _target_rows(t: torch.Tensor):
-    """(address, nbytes) rows of a dense or row-strided tensor in logical order, else None.
-    CUDA rows follow _row_ranges' minimum row size; a CPU row is one pread of any size."""
-    from ..shm_handler import _row_ranges
-
-    if t.is_contiguous():
-        return [(t.data_ptr(), t.numel() * t.element_size())]
-    rows = _row_ranges(t, 0) if t.is_cuda else _row_ranges(t, 0, min_row_bytes=1)
-    return None if rows is None else [(p, n) for p, _, n in rows]
-
-
 def _plan_reads(items, storage_data, state_dict_metadata, resolve):
     """Split DCP read items into direct pieces and fallback items.  Returns (cuda, host,
     slow, targets): cuda / host are (address, relative path, file offset, nbytes) pieces
     into CUDA / CPU targets; slow are the items _load_item reads (BYTE_IO, a dtype
     mismatch, a target that is neither dense nor row-strided, a box above the row cap);
     targets are (item, resolved target) of the direct items, to commit once filled."""
-    from ..shm_handler import _pair_rows
-
     cuda, host, slow, targets = [], [], [], []
     for item in items:
         info = storage_data[item.storage_index]
@@ -655,17 +648,6 @@ def _plan_reads(items, storage_data, state_dict_metadata, resolve):
     return cuda, host, slow, targets
 
 
-def _pread_bytes(fd: int, nbytes: int, offset: int) -> bytes:
-    parts, got = [], 0
-    while got < nbytes:
-        b = os.pread(fd, nbytes - got, offset + got)
-        if not b:
-            raise OSError(f"short read at file offset {offset + got}")
-        parts.append(b)
-        got += len(b)
-    return b"".join(parts)
-
-
 class FileDmaReader(FileReader):
     """FileReader whose tensor items skip the per-item pageable copy: every CUDA item of
     the plan is read through the library's file fill into the HBM arena and scattered by
@@ -674,71 +656,37 @@ class FileDmaReader(FileReader):
     resharding asks for is read as rows of its stored chunk, never the whole chunk.  The
     bytes are those FileReader gives; everything else (BYTE_IO, dtype mismatches, targets
     that are neither dense nor row-strided, boxes above the row cap) goes through
-    FileReader's path.  A shard file too short for any item raises ValueError before a
-    target changes.  `last_read_stats` describes the last read_data."""
+    FileReader's path.  A shard file too short for any item (ShortFileError, a
+    ValueError) or CUDA targets on more than one device (ValueError) raise before a target
+    changes.  `last_read_stats` describes the last read_data."""
 
     def __init__(self, path: Union[str, os.PathLike]) -> None:
         super().__init__(path)
         self.last_read_stats: Dict[str, float] = {}
 
     def read_data(self, plan: LoadPlan, planner: LoadPlanner) -> Future[None]:
-        from ..shm_handler import _pread_into, _restore_file_groups
-
         t0 = time.perf_counter()
         cuda, host, slow, targets = _plan_reads(plan.items, self.storage_data,
                                                 self.state_dict_metadata, planner.resolve_tensor)
-        # the highest byte every file must hold: direct pieces and whole fallback chunks
-        need: Dict[str, int] = {}
-        for _, path, f, n in cuda + host:
-            need[path] = max(need.get(path, 0), f + n)
-        for item in slow:
-            info = self.storage_data[item.storage_index]
-            need[info.relative_path] = max(need.get(info.relative_path, 0),
-                                           info.offset + info.length)
-        stats = {"device_bytes": 0.0, "host_bytes": 0.0, "fallback_items": len(slow),
-                 "files": len(need), "plans": 0, "read_ms": 0.0, "scatter_ms": 0.0,
-                 "wall_ms": 0.0}
-        fds: Dict[str, int] = {}
-        try:
-            for path in sorted(need):
-                fds[path] = os.open(self.path / path, os.O_RDONLY)
-                size = os.fstat(fds[path]).st_size
-                if size < need[path]:  # refuse before any target changes
-                    raise ValueError(f"{self.path / path}: the read items need bytes up to "
-                                     f"file offset {need[path]}, the file ends at {size}")
-            with torch.no_grad():
-                if cuda:
-                    # the files' virtual concatenation: file k starts where file k-1 ends
-                    paths = sorted({p for _, p, _, _ in cuda})
-                    bases, b = {}, 0
-                    for path in paths:
-                        bases[path] = b
-                        b += need[path]
-                    ranges = sorted(((a, bases[p] + f, n) for a, p, f, n in cuda),
-                                    key=lambda r: r[1])
-                    dev = next(t for _, t in targets if t.is_cuda).device
-                    stats["plans"] = _restore_file_groups(
-                        ranges, dev.index if dev.index is not None else torch.cuda.current_device(),
-                        None, lambda pl, s: pl.restore_files_async(
-                            [fds[p] for p in paths], [bases[p] for p in paths], s), stats)
-                t1 = time.perf_counter()
-                for a, path, f, n in host:
-                    _pread_into(fds[path], a, n, f)
-                stats["host_bytes"] = float(sum(n for _, _, _, n in host))
-                for item in slow:
-                    info = self.storage_data[item.storage_index]
-                    item_bytes = io.BytesIO(_pread_bytes(fds[info.relative_path],
-                                                         info.length, info.offset))
-                    md = None
-                    if item.type != LoadItemType.BYTE_IO:
-                        md = self.state_dict_metadata[item.storage_index.fqn]
-                    _load_item(item, item_bytes, planner, md)
-                stats["read_ms"] += (time.perf_counter() - t1) * 1e3
-            for item, target in targets:
-                planner.commit_tensor(item, target)
-        finally:
-            for fd in fds.values():
-                os.close(fd)
+        chunks = [self.storage_data[item.storage_index] for item in slow]
+        with _open_files(self.path, cuda + host,
+                         [(c.relative_path, c.offset + c.length) for c in chunks]) as fds, \
+                torch.no_grad():
+            stats = _read_pieces(fds, cuda, host, [(item.storage_index.fqn, t.device)
+                                                   for item, t in targets if t.is_cuda])
+            t1 = time.perf_counter()
+            for item, info in zip(slow, chunks):
+                item_bytes = io.BytesIO(bytes(info.length))
+                with item_bytes.getbuffer() as view:
+                    _pread_into(fds[info.relative_path], view, info.offset)
+                md = None
+                if item.type != LoadItemType.BYTE_IO:
+                    md = self.state_dict_metadata[item.storage_index.fqn]
+                _load_item(item, item_bytes, planner, md)
+            stats["read_ms"] += (time.perf_counter() - t1) * 1e3
+        for item, target in targets:
+            planner.commit_tensor(item, target)
+        stats["fallback_items"] = len(slow)
         stats["wall_ms"] = (time.perf_counter() - t0) * 1e3
         self.last_read_stats = stats
         fut: Future = Future()

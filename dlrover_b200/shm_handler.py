@@ -27,7 +27,9 @@ from __future__ import annotations
 
 import atexit
 import bisect
+import contextlib
 import copy
+import ctypes
 import json
 import os
 import pickle
@@ -256,48 +258,25 @@ def _local_boxes(value):
 
 def _box_ranges(local: torch.Tensor, offsets, full_shape, full_off: int):
     """(tensor piece, segment offset, nbytes) for a local box of a row-major full tensor
-    that starts at `full_off` in the segment.  A dim-0 shard (every other dim complete) is
-    one contiguous range; anything else is one range per run of complete trailing dims."""
-    es = local.element_size()
+    that starts at `full_off` in the segment: the box's rows (_view_rows) at the full
+    tensor's strides.  A dim-0 shard (every other dim complete) is one contiguous range;
+    anything else is one range per run of complete trailing dims.  Each piece is a row of
+    the local tensor in its own dtype."""
     shape = tuple(local.shape)
     if local.numel() == 0:
         return []
     if len(shape) != len(full_shape):
         raise ValueError(f"local shard {shape} vs full tensor {tuple(full_shape)}")
-    # trailing dims that the box covers completely
-    k = len(shape)
-    while k > 1 and shape[k - 1] == full_shape[k - 1]:
-        k -= 1
-    # the run = dims [k-1:] of the box (dim k-1 may be partial), rows = dims [:k-1]
-    stride = [1] * len(full_shape)
-    for d in range(len(full_shape) - 2, -1, -1):
-        stride[d] = stride[d + 1] * full_shape[d + 1]
-    run_elems = 1
-    for d in range(max(k - 1, 0), len(shape)):
-        run_elems *= shape[d]
-    lead = shape[:max(k - 1, 0)]
-    n_rows = 1
-    for d in lead:
-        n_rows *= d
-    if n_rows > (1 << 16):
+    strides, s = [], 1
+    for n in reversed(full_shape):
+        strides.insert(0, s)
+        s *= n
+    first = sum(o * st for o, st in zip(offsets, strides))
+    rows = _view_rows(shape, strides, first, local.element_size())
+    if rows is None:
         raise ValueError("local shard decomposes into too many rows")
-    local = local.detach()
-    if not local.is_contiguous():
-        local = local.contiguous()
-    flat = local.reshape(n_rows, run_elems) if n_rows > 1 else local.reshape(1, run_elems)
-    out = []
-    idx = [0] * len(lead)
-    for r in range(n_rows):
-        elem = sum((offsets[d] + idx[d]) * stride[d] for d in range(len(lead)))
-        if k >= 1:
-            elem += offsets[k - 1] * stride[k - 1] if len(shape) else 0
-        out.append((flat[r], full_off + elem * es, run_elems * es))
-        for d in range(len(lead) - 1, -1, -1):
-            idx[d] += 1
-            if idx[d] < lead[d]:
-                break
-            idx[d] = 0
-    return out
+    flat = local.detach().contiguous().reshape(len(rows), -1)
+    return [(flat[r], full_off + o, n) for r, (o, n) in enumerate(rows)]
 
 
 def plan_layout_full_from_shards(state_dict):
@@ -425,40 +404,57 @@ def _numa_remote_share(device_index: int) -> int:
         return 0
 
 
-def _row_ranges(t: torch.Tensor, off: int, max_rows: int = 1 << 16, min_row_bytes: int = 256):
-    """A non-contiguous tensor whose trailing dims are dense ("row-strided": w[:, :k],
-    w[::2], a transposed-then-sliced view...) as one (ptr, offset, nbytes) range per dense
-    row, in logical (row-major) order — exactly the bytes `shm.copy_(t)` deposits
-    (reference ckpt_saver.py:228-231) without a device-side .contiguous() copy.
-    None when the rows would be too many / too small (the caller repacks then)."""
-    es = t.element_size()
-    sizes, strides = list(t.shape), list(t.stride())
-    k = len(sizes)  # dims [k:] form the dense row
-    expect = 1
+def _view_rows(shape, stride, first: int, es: int, max_rows: int = 1 << 16,
+               min_row_bytes: int = 0):
+    """The bytes of a strided view in logical (row-major) order, as (byte offset, nbytes)
+    rows starting from element `first`: one row for a dense view, one per dense row when
+    the trailing dims are dense ("row-strided"; size-1 dims count as dense).  None when
+    there would be more than `max_rows` rows, rows under `min_row_bytes`, or a negative
+    stride among the row dims.  The one row walker: tensors, boxes of row-major tensors
+    and views stored in files all map onto it."""
+    sizes, strides = list(shape), list(stride)
+    k, expect = len(sizes), 1  # dims [k:] form the dense row
     while k > 0 and (sizes[k - 1] == 1 or strides[k - 1] == expect):
         expect *= sizes[k - 1]
         k -= 1
-    row_bytes = expect * es
     n_rows = 1
     for d in range(k):
         n_rows *= sizes[d]
-    if k == 0 or row_bytes < min_row_bytes or n_rows > max_rows or any(
-            st < 0 for st in strides[:k]):
+    if expect * es < min_row_bytes or n_rows > max_rows or any(s < 0 for s in strides[:k]):
         return None
-    base = t.data_ptr()
-    out = []
-    idx = [0] * k
-    for r in range(n_rows):
-        elem = 0
-        for d in range(k):
-            elem += idx[d] * strides[d]
-        out.append((base + elem * es, off + r * row_bytes, row_bytes))
+    out, idx = [], [0] * k
+    for _ in range(n_rows):
+        out.append(((first + sum(i * s for i, s in zip(idx, strides))) * es, expect * es))
         for d in range(k - 1, -1, -1):
             idx[d] += 1
             if idx[d] < sizes[d]:
                 break
             idx[d] = 0
     return out
+
+
+def _row_ranges(t: torch.Tensor, off: int, max_rows: int = 1 << 16, min_row_bytes: int = 256):
+    """A non-contiguous tensor whose trailing dims are dense ("row-strided": w[:, :k],
+    w[::2], a transposed-then-sliced view...) as one (ptr, offset, nbytes) range per dense
+    row, in logical (row-major) order — exactly the bytes `shm.copy_(t)` deposits
+    (reference ckpt_saver.py:228-231) without a device-side .contiguous() copy.
+    None for a dense tensor and when the rows would be too many / too small (the caller
+    takes the tensor whole or repacks it then)."""
+    rows = _view_rows(t.shape, t.stride(), 0, t.element_size(), max_rows, min_row_bytes)
+    if rows is None or len(rows) == 1:  # one row: the tensor is dense
+        return None
+    base = t.data_ptr()
+    return [(base + o, off + r * n, n) for r, (o, n) in enumerate(rows)]
+
+
+def _target_rows(t: torch.Tensor):
+    """(address, nbytes) rows of a dense or row-strided restore target in logical order,
+    else None.  A dense tensor is one row; CUDA rows follow _row_ranges' minimum row size
+    (the scatter kernels); a CPU row is one pread of any size."""
+    if t.is_contiguous():
+        return [(t.data_ptr(), t.numel() * t.element_size())]
+    rows = _row_ranges(t, 0) if t.is_cuda else _row_ranges(t, 0, min_row_bytes=1)
+    return None if rows is None else [(p, n) for p, _, n in rows]
 
 
 # kind of the non-finite scan per dtype: complex as its float components; integers, bool
@@ -1846,31 +1842,14 @@ class SharedMemoryHandler:
 
 
 # -- restore from a torch.save file ----------------------------------------------------
-def _view_rows(shape, stride, first: int, es: int, max_rows: int = 1 << 16):
-    """The bytes of a strided view in logical (row-major) order, as (offset, nbytes) rows
-    starting from element `first`: one row for a dense view, one per dense row when the
-    trailing dims are dense ("row-strided"); None for any other view."""
-    sizes, strides = list(shape), list(stride)
-    k, expect = len(sizes), 1
-    while k > 0 and (sizes[k - 1] == 1 or strides[k - 1] == expect):
-        expect *= sizes[k - 1]
-        k -= 1
-    if k == 0:
-        return [(first * es, expect * es)]
-    n_rows = 1
-    for d in range(k):
-        n_rows *= sizes[d]
-    if (expect == 1 and sizes[-1] != 1) or n_rows > max_rows or any(s < 0 for s in strides[:k]):
-        return None
-    out, idx = [], [0] * k
-    for _ in range(n_rows):
-        out.append(((first + sum(i * s for i, s in zip(idx, strides))) * es, expect * es))
-        for d in range(k - 1, -1, -1):
-            idx[d] += 1
-            if idx[d] < sizes[d]:
-                break
-            idx[d] = 0
-    return out
+# Both storage readers (restore_file_into here, FileDmaReader for DCP shard files) turn
+# their leaves into (target address, file, file offset, n) pieces and share the rest:
+# _open_files checks every file's length before a byte moves, _read_pieces reads.
+
+
+class ShortFileError(OSError, ValueError):
+    """A file ends before the last byte a restore reads from it; raised before any target
+    changes.  An OSError for restore_file_into, a ValueError for a DCP StorageReader."""
 
 
 def _pair_rows(src, dst):
@@ -1889,33 +1868,15 @@ def _pair_rows(src, dst):
     return out
 
 
-def _file_ranges(index, pairs):
-    """(target address, file offset, nbytes, leaf path) of every leaf of `pairs`, sorted by
-    file offset.  A range that repeats bytes of another one into the same place (tied
-    weights: two leaves, one storage in the file and one in the model) is dropped."""
-    ranges = []
-    for name, t, leaf in pairs:
-        es = t.element_size()
-        src = _view_rows(leaf.shape, leaf.stride, leaf.storage_offset, es)
-        if src is None:
-            raise ValueError(f"{name}: the file holds a view that is neither dense nor "
-                             f"row-strided (shape {leaf.shape}, stride {leaf.stride}) in "
-                             f"{index.path}")
-        src = [(leaf.file_offset + o, n) for o, n in src]
-        if t.is_contiguous():
-            dst = [(t.data_ptr(), t.numel() * es)]
-        else:
-            rows = _row_ranges(t, 0)
-            if rows is None:
-                raise ValueError(f"{name}: restore needs dense or row-strided CUDA targets "
-                                 f"(got shape {tuple(t.shape)}, strides {t.stride()})")
-            dst = [(p, n) for p, _, n in rows]
-        ranges += [(p, f, n, name) for p, f, n in _pair_rows(src, dst)]
-    ranges.sort(key=lambda r: (r[1], -r[2]))
-    out, live = [], []  # live: kept ranges that reach past the current file offset
-    for r in ranges:
-        live = [k for k in live if k[1] + k[2] > r[1]]
-        if any(r[1] + r[2] <= f + n and r[0] - p == r[1] - f for p, f, n, _ in live):
+def _unique_pieces(pieces):
+    """(address, file, file offset, n) pieces sorted by file and offset, without those that
+    repeat bytes of another piece into the same place (tied weights: two leaves, one
+    storage in the file and one in the model)."""
+    out, live = [], []  # live: kept pieces of the same file that reach past the offset
+    for r in sorted(pieces, key=lambda r: (r[1], r[2], -r[3])):
+        a, f, o, n = r
+        live = [k for k in live if k[1] == f and k[2] + k[3] > o]
+        if any(o + n <= ko + kn and a - ka == o - ko for ka, _, ko, kn in live):
             continue
         out.append(r)
         live.append(r)
@@ -1938,18 +1899,17 @@ def _disjoint_groups(ranges):
 
 
 def _restore_file_groups(ranges, device_index: int, stream, enqueue, stats) -> int:
-    """Restore CUDA (address, file offset, nbytes, ...) ranges, sorted by file offset,
-    through the arena of `device_index`: one mapped plan per _disjoint_groups group, whose
-    file fill enqueue(plan, stream) starts (fc_restore_file_async or
-    fc_restore_files_async).  Adds device_bytes, read_ms and scatter_ms to `stats`; returns
-    the number of plans."""
+    """Restore CUDA (address, file offset, nbytes) ranges, sorted by file offset, through
+    the arena of `device_index`: one mapped plan per _disjoint_groups group, whose file
+    fill enqueue(plan, stream) starts.  Adds device_bytes, read_ms and scatter_ms to
+    `stats`; returns the number of plans."""
     ctx = native.get_context(device_index)
     if stream is None:
         stream = torch.cuda.current_stream(device_index)
     groups = _disjoint_groups(ranges)
     for group in groups:
         ptrs, arena, foffs, lens, a = [], [], [], [], 0
-        for p, f, n, *_ in group:
+        for p, f, n in group:
             a += (p - a) % 16  # congruent to the target mod 16: the bulk kernel
             ptrs.append(p)
             arena.append(a)
@@ -1971,16 +1931,77 @@ def _restore_file_groups(ranges, device_index: int, stream, enqueue, stats) -> i
     return len(groups)
 
 
-def _pread_into(fd: int, address: int, nbytes: int, offset: int):
-    import ctypes
-
-    view = memoryview((ctypes.c_char * nbytes).from_address(address)).cast("B")
+def _pread_into(fd: int, buf, offset: int):
+    """Fill the writable buffer `buf` from `fd` at `offset`."""
+    view = memoryview(buf).cast("B")
     got = 0
-    while got < nbytes:
+    while got < len(view):
         n = os.preadv(fd, [view[got:]], offset + got)
         if n <= 0:
             raise OSError(f"short read at file offset {offset + got}")
         got += n
+
+
+@contextlib.contextmanager
+def _open_files(root, pieces, more=()):
+    """Open every file that (address, file, file offset, n) `pieces` and the (file, end)
+    pairs of `more` name, relative to `root`, and check each with fstat against the
+    highest byte they read from it before any byte moves (ShortFileError).  Yields
+    {file: fd}; every fd is closed on the way out."""
+    need: Dict[Any, int] = {}
+    for f, end in [(f, o + n) for _, f, o, n in pieces] + list(more):
+        need[f] = max(need.get(f, 0), end)
+    fds: Dict[Any, int] = {}
+    try:
+        for f in sorted(need):
+            path = os.path.join(root, f)
+            fds[f] = os.open(path, os.O_RDONLY)
+            size = os.fstat(fds[f]).st_size
+            if size < need[f]:
+                raise ShortFileError(f"{path}: the restore reads bytes up to file offset "
+                                     f"{need[f]}, the file ends at {size}")
+        yield fds
+    finally:
+        for fd in fds.values():
+            os.close(fd)
+
+
+def _read_pieces(fds, cuda, host, devices, stream=None) -> Dict[str, float]:
+    """Read (address, file, file offset, n) pieces from the files `_open_files` opened.
+    CUDA pieces: their targets, (name, device) in `devices`, must share one device; the
+    pieces, sorted and without repeats (_unique_pieces), go through the arena in one file
+    fill per _disjoint_groups group (fc_restore_files_async over the files' virtual
+    concatenation, file k owning [bases[k], bases[k+1]); one file is n = 1, base 0).  CPU
+    pieces are pread straight in.  Returns device_bytes, host_bytes, read_ms, scatter_ms,
+    plans and files."""
+    stats = {"device_bytes": 0.0, "host_bytes": 0.0, "read_ms": 0.0, "scatter_ms": 0.0,
+             "plans": 0, "files": len(fds)}
+    for name, d in devices:
+        if d != devices[0][1]:
+            raise ValueError(f"{name}: all CUDA leaves must live on one device; "
+                             f"got {devices[0][1]} and {d}")
+    if cuda:
+        dev = devices[0][1]
+        cuda = _unique_pieces(cuda)
+        ends: Dict[Any, int] = {}  # in file order: the pieces are sorted by file
+        for _, f, o, n in cuda:
+            ends[f] = max(ends.get(f, 0), o + n)
+        bases, b = {}, 0
+        for f, end in ends.items():
+            bases[f] = b
+            b += end
+        ranges = [(a, bases[f] + o, n) for a, f, o, n in cuda]
+        stats["plans"] = _restore_file_groups(
+            ranges, dev.index if dev.index is not None else torch.cuda.current_device(),
+            stream, lambda plan, s: plan.restore_files_async(
+                [fds[f] for f in bases], list(bases.values()), s), stats)
+    t0 = time.perf_counter()
+    host = _unique_pieces(host)
+    for a, f, o, n in host:
+        _pread_into(fds[f], (ctypes.c_char * n).from_address(a), o)
+    stats["host_bytes"] = float(sum(n for _, _, _, n in host))
+    stats["read_ms"] += (time.perf_counter() - t0) * 1e3
+    return stats
 
 
 def restore_file_into(path: str, target, stream=None, strict: bool = True,
@@ -1990,10 +2011,10 @@ def restore_file_into(path: str, target, stream=None, strict: bool = True,
     indexed without reading its payload (`torch_file_index.index_file`, torch's
     weights_only unpickler; pass `index` to reuse one).  CUDA leaves: the library preads
     the file through pinned bounce slots into the arena and scatters it with the unpack
-    kernels (fc_restore_file_async); CPU leaves are pread straight into the tensors.
-    Non-tensor leaves of the file are ignored.  On a short file or a failed read nothing
-    is scattered and the call raises.  The incremental-save baseline and the arena image
-    are forgotten, as by every restore.
+    kernels (fc_restore_files_async); CPU leaves are pread straight into the tensors.
+    Non-tensor leaves of the file are ignored.  On a short file (ShortFileError, an
+    OSError) or a failed read nothing is scattered and the call raises.  The
+    incremental-save baseline and the arena image are forgotten, as by every restore.
 
     Replaces `sd = torch.load(path, map_location="cpu"); model.load_state_dict(sd)`.
     stats: device_bytes, host_bytes, read_ms, scatter_ms, wall_ms."""
@@ -2002,45 +2023,34 @@ def restore_file_into(path: str, target, stream=None, strict: bool = True,
     t0 = time.perf_counter()
     if index is None:
         index = index_file(path)
-    pairs = _match_tree(target, index.tree, TensorLeaf, (list, tuple), strict)
-    dev_pairs = [p for p in pairs if p[1].is_cuda]
-    host_pairs = [p for p in pairs if not p[1].is_cuda]
-    stats = {"device_bytes": 0.0, "host_bytes": 0.0, "read_ms": 0.0, "scatter_ms": 0.0,
-             "wall_ms": 0.0}
-    fd = os.open(path, os.O_RDONLY)
-    try:
-        size = os.fstat(fd).st_size
-        # strided CPU targets are read into a dense copy first (one per target tensor:
-        # tied leaves share it), then torch copies the strides
-        staging = {}
-        for _, t, _ in host_pairs:
-            if not t.is_contiguous() and id(t) not in staging:
+    cuda, host, devices = [], [], []
+    staging = {}  # CPU targets without dense rows: read into a dense copy, then copy_
+    for name, t, leaf in _match_tree(target, index.tree, TensorLeaf, (list, tuple), strict):
+        shape, stride = leaf.shape, leaf.stride
+        src = _view_rows(shape, stride, leaf.storage_offset, t.element_size())
+        if src is None or (shape and shape[-1] != 1 and stride[-1] != 1):
+            raise ValueError(f"{name}: the file holds a view that is neither dense nor "
+                             f"row-strided (shape {shape}, stride {stride}) in {index.path}")
+        dst = _target_rows(t)
+        if dst is None and t.is_cuda:
+            raise ValueError(f"{name}: restore needs dense or row-strided CUDA targets "
+                             f"(got shape {tuple(t.shape)}, strides {t.stride()})")
+        if dst is None:  # one dense copy per target tensor: tied leaves share it
+            if id(t) not in staging:
                 staging[id(t)] = (t, torch.empty(t.shape, dtype=t.dtype))
-        host = _file_ranges(index, [(n, staging[id(t)][1] if id(t) in staging else t, leaf)
-                                    for n, t, leaf in host_pairs])
-        dev_ranges = _file_ranges(index, dev_pairs)
-        end = max((f + n for _, f, n, _ in host + dev_ranges), default=0)
-        if end > size:  # a truncated file: refuse before any tensor changes
-            raise OSError(f"{path}: the leaves need bytes up to file offset {end}, the file "
-                          f"ends at {size}")
-        with torch.no_grad():
-            if dev_pairs:
-                dev = dev_pairs[0][1].device
-                for name, t, _ in dev_pairs:
-                    if t.device != dev:
-                        raise ValueError(f"{name}: all CUDA leaves must live on one device; "
-                                         f"got {dev} and {t.device}")
-                device_index = dev.index if dev.index is not None else torch.cuda.current_device()
-                _restore_file_groups(dev_ranges, device_index, stream,
-                                     lambda plan, s: plan.restore_file_async(fd, s), stats)
-            t1 = time.perf_counter()
-            for p, f, n, _ in host:
-                _pread_into(fd, p, n, f)
-            for t, s in staging.values():
-                t.copy_(s)
-            stats["read_ms"] += (time.perf_counter() - t1) * 1e3
-            stats["host_bytes"] = float(sum(n for _, _, n, _ in host))
-    finally:
-        os.close(fd)
+            dst = _target_rows(staging[id(t)][1])
+        if t.is_cuda:
+            devices.append((name, t.device))
+        (cuda if t.is_cuda else host).extend(
+            (p, path, leaf.file_offset + f, n) for p, f, n in _pair_rows(src, dst))
+    with _open_files("", cuda + host) as fds, torch.no_grad():
+        got = _read_pieces(fds, cuda, host, devices, stream)
+        t1 = time.perf_counter()
+        for t, s in staging.values():
+            t.copy_(s)
+    stats = {k: got[k] for k in ("device_bytes", "host_bytes", "read_ms", "scatter_ms")}
+    stats["read_ms"] += (time.perf_counter() - t1) * 1e3
     stats["wall_ms"] = (time.perf_counter() - t0) * 1e3
     return stats
+
+
