@@ -74,10 +74,29 @@ class FsdpShardCheckpointer(Checkpointer):
             _dispatch(self._engine, storage_type, step, state_dict, {_MODEL: path})
 
     def load_checkpoint(self, model, optimizer, resume_path=""):
+        return self._load(model, optimizer, lambda: self._engine.load(resume_path))
+
+    def rollback_checkpoint(self, model, optimizer):
+        """load_checkpoint from this process's own last memory checkpoint, for a rollback
+        (a loss spike, a NaN step, a survivor resetting to the last consistent step).
+        Each of the two passes (model, optimizer) scatters its tensor items from the HBM
+        snapshot of that save when every rank's snapshot covers them: nothing crosses
+        PCIe.  Otherwise every rank reads that pass from its segment, as load_checkpoint
+        does; the bytes are the same either way.  FSDP hands the sharded optimizer state
+        to save_checkpoint as host copies (ShardedOptimStateDictConfig's default
+        offload_to_cpu=True), so it is never in the snapshot: its pass reads the segment,
+        and like every restore from the segment it retires the snapshot and the
+        incremental baseline.  Returns what load_checkpoint returns, or {} when the ranks
+        hold no common step in memory (storage is not consulted).
+        engine.last_rollback_stats() tells which path each pass took.  Every rank must
+        call it."""
+        return self._load(model, optimizer, self._engine.rollback_reader)
+
+    def _load(self, model, optimizer, get_reader):
         with FSDP.state_dict_type(model, StateDictType.SHARDED_STATE_DICT):
             # the optimizer state cannot be loaded in the same pass as the model
             state_dict = {"model": model.state_dict(), "step": 0}
-            reader = self._engine.load(resume_path)
+            reader = get_reader()
             if not reader:
                 return {}
             _dcp_load(state_dict, reader)

@@ -489,17 +489,23 @@ class SharedMemoryReader(StorageReader):
             return None
         return target, info.offset, info.length
 
-    def read_data(self, plan: LoadPlan, planner: LoadPlanner) -> Future[None]:
-        self.shm_handler.wait_pending()
-        if self.shm_handler.shared_memory is None:
-            self.shm_handler.init_shared_memory()
-        fast = []  # (read_item, target, offset, nbytes)
+    def _split_items(self, plan: LoadPlan, planner: LoadPlanner):
+        """(fast, slow): fast are (read_item, target, offset, nbytes) of the items
+        _device_fast_path takes, slow are (read_item, storage info) of the others."""
+        fast, slow = [], []
         for read_item in plan.items:
             info = self.storage_data[read_item.storage_index]
             hit = self._device_fast_path(read_item, info, planner)
             if hit is not None:
                 fast.append((read_item,) + hit)
-                continue
+            else:
+                slow.append((read_item, info))
+        return fast, slow
+
+    def _load_slow_items(self, slow, planner: LoadPlanner):
+        """Each item one by one: non-sharded entries from the `no_shard_data` copy, the
+        rest from the segment."""
+        for read_item, info in slow:
             pickled = False
             if not read_item.storage_index.offset:
                 # non-sharded entry: taken from the broadcast copy, not the segment
@@ -519,6 +525,13 @@ class SharedMemoryReader(StorageReader):
             if read_item.type != LoadItemType.BYTE_IO:
                 md = self.state_dict_metadata[read_item.storage_index.fqn]
             _load_item(read_item, item_bytes, planner, md, pickled=pickled)
+
+    def read_data(self, plan: LoadPlan, planner: LoadPlanner) -> Future[None]:
+        self.shm_handler.wait_pending()
+        if self.shm_handler.shared_memory is None:
+            self.shm_handler.init_shared_memory()
+        fast, slow = self._split_items(plan, planner)
+        self._load_slow_items(slow, planner)
         self.last_fast_items = len(fast)
         if fast:
             self.shm_handler.read_ranges([(t, off, n) for _, t, off, n in fast])
@@ -551,6 +564,61 @@ class SharedMemoryReader(StorageReader):
     @classmethod
     def validate_checkpoint_id(cls, checkpoint_id: Union[str, os.PathLike]) -> bool:
         return True
+
+
+class RollbackReader(SharedMemoryReader):
+    """SharedMemoryReader for a process that saved the in-memory checkpoint itself
+    (FsdpCheckpointEngine.rollback_reader): the fast items are scattered from the HBM
+    arena image of the last full-snapshot save when EVERY rank of `group` holds an image
+    covering its own fast items, so none of their bytes crosses PCIe; otherwise every
+    rank reads them from its segment as SharedMemoryReader does.  The other items take
+    SharedMemoryReader's path either way.  Each read_data makes one all-reduce over
+    `group`: every rank of it must read through such a reader in the same dcp.load.
+
+    last_read_stats: from_image (1.0 / 0.0), fast_items, slow_items, device_bytes,
+    fill_ms, scatter_ms, wall_ms of the last read_data; `passes` holds those of every
+    read_data since the engine handed the reader out."""
+
+    def __init__(self, shm_handler: SharedMemoryHandler, group=None) -> None:
+        super().__init__(shm_handler)
+        self.group = group
+        self.last_read_stats: Dict[str, float] = {}
+        self.passes: List[Dict[str, float]] = []
+
+    def read_data(self, plan: LoadPlan, planner: LoadPlanner) -> Future[None]:
+        t0 = time.perf_counter()
+        handler = self.shm_handler
+        error = None
+        try:
+            handler.wait_pending()
+            if handler.shared_memory is None:
+                handler.init_shared_memory()
+            fast, slow = self._split_items(plan, planner)
+            ranges = [(t, off, n) for _, t, off, n in fast]
+            covered = handler.image_covers_ranges(ranges)
+        except Exception as e:  # vote first: the other ranks are on their way to the collective
+            error, covered = e, False
+        image = all_reduce_flags(self.group, [0 if covered else 1])[0] == 0
+        if error is not None:
+            raise error
+        self._load_slow_items(slow, planner)
+        self.last_fast_items = len(fast)
+        stats = {"from_image": float(image), "fast_items": float(len(fast)),
+                 "slow_items": float(len(slow)), "device_bytes": 0.0, "fill_ms": 0.0,
+                 "scatter_ms": 0.0}
+        if fast:
+            got = handler.read_ranges(ranges, image_first=image)
+            stats["from_image"] = got.get("from_image", 0.0)
+            for key in ("device_bytes", "fill_ms", "scatter_ms"):
+                stats[key] = got[key]
+            for read_item, target, _, _ in fast:
+                planner.commit_tensor(read_item, target)
+        stats["wall_ms"] = (time.perf_counter() - t0) * 1e3
+        self.last_read_stats = stats
+        self.passes.append(stats)
+        fut: Future = Future()
+        fut.set_result(None)
+        return fut
 
 
 class FileReader(StorageReader):
@@ -738,6 +806,7 @@ class FsdpCheckpointEngine(CheckpointEngine):
         self._shm_writer = SharedMemoryWriter(shm_handler=self._shm_handler,
                                               blocking=not self._async_drain)
         self._shm_reader = SharedMemoryReader(self._shm_handler)
+        self._rollback_reader = RollbackReader(self._shm_handler, self._saver_group)
         self._plan_cache: Optional[Dict[str, Any]] = None
         self._published_meta: Dict[str, Any] = {}
         self.last_save_reused_plan = False
@@ -977,6 +1046,29 @@ class FsdpCheckpointEngine(CheckpointEngine):
             logger.info(f"Create a storage reader with path {resume_path}.")
             return FileDmaReader(resume_path) if self.storage_dma else FileReader(resume_path)
         return None
+
+    def rollback_reader(self) -> Optional[RollbackReader]:
+        """A StorageReader that rolls this process back to its own last memory checkpoint
+        (after a loss spike, a NaN step, or a survivor resetting to the last consistent
+        step): the memory branch of load(), whose tensor items are scattered from the HBM
+        arena image when every rank still holds one (RollbackReader).  None when the ranks
+        do not all hold the same, completely written step in memory; there is no fallback
+        to storage.  Every rank must call it."""
+        self.wait_memory_save()
+        config = self._shm_handler.get_checkpoint_config(CheckpointConfig())
+        # a segment still being written counts as no checkpoint, on every rank alike
+        step = 0 if config.writing_shm else config.step
+        if not verify_all_rank_step_consistent(self._saver_group, step) or step <= 0:
+            return None
+        logger.info(f"Create a rollback reader with step {step}.")
+        self._rollback_reader.passes = []
+        return self._rollback_reader
+
+    def last_rollback_stats(self) -> List[Dict[str, float]]:
+        """RollbackReader.last_read_stats of every dcp.load pass through the reader the
+        last rollback_reader() returned, in order (FsdpShardCheckpointer.
+        rollback_checkpoint: the model, then the optimizer)."""
+        return list(self._rollback_reader.passes)
 
     def _get_track_resume_path(self):
         tracker = os.path.join(self.checkpoint_dir, CheckpointConstant.TRACER_FILE_NAME)

@@ -1672,15 +1672,23 @@ class SharedMemoryHandler:
             stats["host_bytes"] = self._restore_host_leaves(host_pairs)
             if device_ranges:
                 stager, plan, stream = self._restore_plan(device_ranges, stream)
-                got = self._run_rollback(stager, plan, stream) if image_first else None
-                if got is None and coop is not None:
-                    got = self._run_restore_cooperative(stager, plan, stream, coop)
-                elif got is None:
-                    got = self._run_restore(stager, plan, stream, pin_after=pin_after)
-                    if image_first:
-                        got["from_image"] = self.last_restore_stats["from_image"] = 0.0
-                stats.update(got)
+                stats.update(self._restore_device(stager, plan, stream, image_first, coop,
+                                                  pin_after))
         return stats
+
+    def _restore_device(self, stager: _DeviceStager, plan, stream, image_first: bool,
+                        coop=None, pin_after: bool = True) -> Dict[str, float]:
+        """The restore of a built plan: from the arena image when image_first and it
+        covers the plan, else from the segment (cooperatively when coop is given).
+        With image_first the stats carry "from_image" (1.0 / 0.0)."""
+        got = self._run_rollback(stager, plan, stream) if image_first else None
+        if got is None and coop is not None:
+            got = self._run_restore_cooperative(stager, plan, stream, coop)
+        elif got is None:
+            got = self._run_restore(stager, plan, stream, pin_after=pin_after)
+            if image_first:
+                got["from_image"] = self.last_restore_stats["from_image"] = 0.0
+        return got
 
     def rollback_into(self, target, stream=None, strict: bool = True) -> Dict[str, float]:
         """restore_into for a process that saved the checkpoint itself: after a
@@ -1806,13 +1814,37 @@ class SharedMemoryHandler:
             stager.pin_in_background()  # the next save wants plain DMA
         return dict(stats)
 
-    def read_ranges(self, device_ranges, stream=None) -> Dict[str, float]:
+    def read_ranges(self, device_ranges, stream=None, *,
+                    image_first: bool = False) -> Dict[str, float]:
         """Inverse of write_ranges for CUDA targets: (tensor, segment offset,
         nbytes) triples are filled by one DMA of the covered segment runs into
-        the arena + one scatter kernel into the (contiguous) tensors."""
+        the arena + one scatter kernel into the (contiguous) tensors.
+
+        image_first: scatter from the arena image of this process's last full-snapshot
+        save when it covers the ranges (one kernel, nothing crosses PCIe; see
+        rollback_into), else as above; the stats then carry "from_image" (1.0 / 0.0)."""
         self.wait_pending()
         if not device_ranges:
-            return {"device_bytes": 0.0, "fill_ms": 0.0, "scatter_ms": 0.0}
+            stats = {"device_bytes": 0.0, "fill_ms": 0.0, "scatter_ms": 0.0}
+            if image_first:
+                stats["from_image"] = 0.0
+            return stats
+        stager, plan, stream = self._read_plan(device_ranges, stream)
+        return self._restore_device(stager, plan, stream, image_first)
+
+    def image_covers_ranges(self, device_ranges) -> bool:
+        """Whether read_ranges(device_ranges, image_first=True) would scatter every range
+        from the arena image; moves nothing.  Raises what read_ranges raises for the same
+        ranges.  True when there are no ranges: there is nothing to move."""
+        self.wait_pending()
+        if not device_ranges:
+            return True
+        _, plan, _ = self._read_plan(device_ranges, None)
+        return plan.image_covers(self.shared_memory.dma_address)
+
+    def _read_plan(self, device_ranges, stream):
+        """read_ranges' checks of non-empty (CUDA tensor, segment offset, nbytes) ranges
+        against the mapped segment, then their restore plan (_restore_plan)."""
         self.refresh_mapping()
         if not self.shared_memory:
             raise RuntimeError("the checkpoint segment does not exist")
@@ -1821,8 +1853,7 @@ class SharedMemoryHandler:
                 raise ValueError("read_ranges needs CUDA targets")
             if off + nbytes > self.shared_memory.size or t.numel() * t.element_size() != nbytes:
                 raise ValueError("read_ranges: range does not fit the segment / the tensor")
-        stager, plan, stream = self._restore_plan(device_ranges, stream)
-        return self._run_restore(stager, plan, stream)
+        return self._restore_plan(device_ranges, stream)
 
     # -- queries ------------------------------------------------------------------------
     def no_checkpoint_state(self):
