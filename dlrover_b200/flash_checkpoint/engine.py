@@ -36,7 +36,7 @@ import time
 from abc import ABCMeta, abstractmethod
 from datetime import timedelta
 from multiprocessing import Process
-from typing import Dict, List, Optional
+from typing import Callable, Dict, List, Optional, Tuple
 
 import torch
 import torch.distributed as dist
@@ -124,6 +124,19 @@ def all_reduce_flags(group: Optional[dist.ProcessGroup], flags: List[int]) -> Li
         dist.all_reduce(t, group=group)
         out = [int(v) for v in t.tolist()]
     return out
+
+
+def vote_all_ranks(group: Optional[dist.ProcessGroup],
+                   check: Callable[[], bool]) -> Tuple[bool, Optional[Exception]]:
+    """(every rank of `group` answered True, this rank's exception or None): runs the
+    local check, counts an exception as False, then takes part in ONE all_reduce_flags.
+    The vote runs whatever the check did, so no rank is left waiting in it; what to do
+    with the exception is the caller's choice."""
+    try:
+        mine, error = bool(check()), None
+    except Exception as e:
+        mine, error = False, e
+    return all_reduce_flags(group, [0 if mine else 1])[0] == 0, error
 
 
 def verify_all_rank_step_consistent(group: Optional[dist.ProcessGroup], step):
@@ -876,13 +889,11 @@ class CheckpointEngine(metaclass=ABCMeta):
         (step, stats); stats["from_image"] says which path ran."""
         config = self._shm_handler.get_checkpoint_config(CheckpointConfig())
         passed = verify_all_rank_step_consistent(self._loader_group, config.step)
-        image = False
-        if passed and config.step > 0:
-            try:
-                image = self._shm_handler.can_rollback(target_state_dict, strict=strict)
-            except Exception:
-                image = False  # load_into below raises the same error on this rank
-        if all_reduce_flags(self._loader_group, [0 if image else 1])[0] == 0:
+        # the error is dropped: load_into below raises it on this rank after its own step
+        # collective, where raising now would leave the other ranks waiting
+        image, _ = vote_all_ranks(self._loader_group, lambda: passed and config.step > 0 and
+                                  self._shm_handler.can_rollback(target_state_dict, strict=strict))
+        if image:
             stats = self._shm_handler.rollback_into(target_state_dict, stream=stream,
                                                     strict=strict)
             return config.step, stats

@@ -76,6 +76,7 @@ from .engine import (
     check_all_rank_ready,
     timer,
     verify_all_rank_step_consistent,
+    vote_all_ranks,
 )
 
 try:  # moved around between torch releases
@@ -456,14 +457,50 @@ def _chunk_shape(md: TensorStorageMetadata, read_item: ReadItem):
     return tuple(read_item.lengths)
 
 
-class SharedMemoryReader(StorageReader):
+class _DcpReader(StorageReader):
+    """What the memory and the file readers share: the metadata DCP sets them up with,
+    the StorageReader steps they have nothing to do in, and the hand-over of one stored
+    item's bytes to the planner."""
+
+    def __init__(self) -> None:
+        super().__init__()
+        self.storage_data: Dict[MetadataIndex, _StorageInfo] = {}
+        self.state_dict_metadata: Dict[str, STORAGE_TYPES] = {}
+
+    def _load_stored(self, item: ReadItem, item_bytes: io.BytesIO, planner: LoadPlanner,
+                     pickled: bool = False):
+        """_load_item with the item's TensorStorageMetadata (none for BYTE_IO)."""
+        md = None
+        if item.type != LoadItemType.BYTE_IO:
+            md = self.state_dict_metadata[item.storage_index.fqn]
+        _load_item(item, item_bytes, planner, md, pickled=pickled)
+
+    def set_up_storage_reader(self, metadata: Metadata, is_coordinator: bool, *args,
+                              **kwargs) -> None:
+        self.storage_data = metadata.storage_data
+        self.state_dict_metadata = metadata.state_dict_metadata
+        assert self.storage_data is not None
+
+    def prepare_local_plan(self, plan: LoadPlan) -> LoadPlan:
+        return plan
+
+    def prepare_global_plan(self, global_plan: List[LoadPlan]) -> List[LoadPlan]:
+        return global_plan
+
+    def reset(self, checkpoint_id: Union[str, os.PathLike, None] = None) -> None:
+        pass
+
+    @classmethod
+    def validate_checkpoint_id(cls, checkpoint_id: Union[str, os.PathLike]) -> bool:
+        return True
+
+
+class SharedMemoryReader(_DcpReader):
     """DCP StorageReader over the shared-memory segment."""
 
     def __init__(self, shm_handler: SharedMemoryHandler) -> None:
         super().__init__()
-        self.storage_data: Dict[MetadataIndex, _StorageInfo] = {}
         self.shm_handler = shm_handler
-        self.state_dict_metadata: Dict[str, STORAGE_TYPES] = {}
         self.no_shard_data: Dict[str, STORAGE_TYPES] = {}
         self.last_fast_items = 0  # items of the last read_data served by DMA + scatter
 
@@ -490,8 +527,12 @@ class SharedMemoryReader(StorageReader):
         return target, info.offset, info.length
 
     def _split_items(self, plan: LoadPlan, planner: LoadPlanner):
-        """(fast, slow): fast are (read_item, target, offset, nbytes) of the items
-        _device_fast_path takes, slow are (read_item, storage info) of the others."""
+        """(fast, slow) once this handler's own drain is over and the segment is mapped:
+        fast are (read_item, target, offset, nbytes) of the items _device_fast_path takes,
+        slow are (read_item, storage info) of the others."""
+        self.shm_handler.wait_pending()
+        if self.shm_handler.shared_memory is None:
+            self.shm_handler.init_shared_memory()
         fast, slow = [], []
         for read_item in plan.items:
             info = self.storage_data[read_item.storage_index]
@@ -501,6 +542,15 @@ class SharedMemoryReader(StorageReader):
             else:
                 slow.append((read_item, info))
         return fast, slow
+
+    def _plan_read(self, plan: LoadPlan, planner: LoadPlanner):
+        """(fast, slow, from the image?) of one read_data: this reader always reads the
+        fast items from the segment, and takes part in no collective."""
+        return (*self._split_items(plan, planner), False)
+
+    def _keep_stats(self, stats: Dict[str, float]) -> None:
+        """Takes the stats of each read_data (see RollbackReader.last_read_stats); this
+        reader keeps none of them."""
 
     def _load_slow_items(self, slow, planner: LoadPlanner):
         """Each item one by one: non-sharded entries from the `no_shard_data` copy, the
@@ -521,22 +571,28 @@ class SharedMemoryReader(StorageReader):
                 item_bytes = io.BytesIO(
                     self.shm_handler.shared_memory.buf[info.offset:info.offset + info.length])
             item_bytes.seek(0)
-            md = None
-            if read_item.type != LoadItemType.BYTE_IO:
-                md = self.state_dict_metadata[read_item.storage_index.fqn]
-            _load_item(read_item, item_bytes, planner, md, pickled=pickled)
+            self._load_stored(read_item, item_bytes, planner, pickled=pickled)
 
     def read_data(self, plan: LoadPlan, planner: LoadPlanner) -> Future[None]:
-        self.shm_handler.wait_pending()
-        if self.shm_handler.shared_memory is None:
-            self.shm_handler.init_shared_memory()
-        fast, slow = self._split_items(plan, planner)
+        """The slow items one by one, then every fast item in one read_ranges: from the
+        arena image when _plan_read says so, else DMA from the segment + scatter."""
+        t0 = time.perf_counter()
+        fast, slow, image = self._plan_read(plan, planner)
         self._load_slow_items(slow, planner)
         self.last_fast_items = len(fast)
+        stats = {"from_image": float(image), "fast_items": float(len(fast)),
+                 "slow_items": float(len(slow)), "device_bytes": 0.0, "fill_ms": 0.0,
+                 "scatter_ms": 0.0}
         if fast:
-            self.shm_handler.read_ranges([(t, off, n) for _, t, off, n in fast])
+            got = self.shm_handler.read_ranges([(t, off, n) for _, t, off, n in fast],
+                                               image_first=image)
+            stats["from_image"] = got.get("from_image", 0.0)
+            for key in ("device_bytes", "fill_ms", "scatter_ms"):
+                stats[key] = got[key]
             for read_item, target, _, _ in fast:
                 planner.commit_tensor(read_item, target)
+        stats["wall_ms"] = (time.perf_counter() - t0) * 1e3
+        self._keep_stats(stats)
         fut: Future = Future()
         fut.set_result(None)
         return fut
@@ -545,25 +601,6 @@ class SharedMemoryReader(StorageReader):
         cached = self.shm_handler.metadata.get()
         self.no_shard_data = cached["no_shard_data"]
         return cached["dcp_metadata"]
-
-    def set_up_storage_reader(self, metadata: Metadata, is_coordinator: bool, *args,
-                              **kwargs) -> None:
-        self.storage_data = metadata.storage_data
-        self.state_dict_metadata = metadata.state_dict_metadata
-        assert self.storage_data is not None
-
-    def prepare_local_plan(self, plan: LoadPlan) -> LoadPlan:
-        return plan
-
-    def prepare_global_plan(self, global_plan: List[LoadPlan]) -> List[LoadPlan]:
-        return global_plan
-
-    def reset(self, checkpoint_id: Union[str, os.PathLike, None] = None) -> None:
-        pass
-
-    @classmethod
-    def validate_checkpoint_id(cls, checkpoint_id: Union[str, os.PathLike]) -> bool:
-        return True
 
 
 class RollbackReader(SharedMemoryReader):
@@ -585,51 +622,33 @@ class RollbackReader(SharedMemoryReader):
         self.last_read_stats: Dict[str, float] = {}
         self.passes: List[Dict[str, float]] = []
 
-    def read_data(self, plan: LoadPlan, planner: LoadPlanner) -> Future[None]:
-        t0 = time.perf_counter()
-        handler = self.shm_handler
-        error = None
-        try:
-            handler.wait_pending()
-            if handler.shared_memory is None:
-                handler.init_shared_memory()
+    def _plan_read(self, plan: LoadPlan, planner: LoadPlanner):
+        """The split, and one vote of the group on whether every rank's image covers its
+        fast items (a rank without fast items is covered)."""
+        fast = slow = None
+
+        def covered():
+            nonlocal fast, slow
             fast, slow = self._split_items(plan, planner)
-            ranges = [(t, off, n) for _, t, off, n in fast]
-            covered = handler.image_covers_ranges(ranges)
-        except Exception as e:  # vote first: the other ranks are on their way to the collective
-            error, covered = e, False
-        image = all_reduce_flags(self.group, [0 if covered else 1])[0] == 0
+            return self.shm_handler.image_covers_ranges([(t, off, n) for _, t, off, n in fast])
+
+        image, error = vote_all_ranks(self.group, covered)
         if error is not None:
-            raise error
-        self._load_slow_items(slow, planner)
-        self.last_fast_items = len(fast)
-        stats = {"from_image": float(image), "fast_items": float(len(fast)),
-                 "slow_items": float(len(slow)), "device_bytes": 0.0, "fill_ms": 0.0,
-                 "scatter_ms": 0.0}
-        if fast:
-            got = handler.read_ranges(ranges, image_first=image)
-            stats["from_image"] = got.get("from_image", 0.0)
-            for key in ("device_bytes", "fill_ms", "scatter_ms"):
-                stats[key] = got[key]
-            for read_item, target, _, _ in fast:
-                planner.commit_tensor(read_item, target)
-        stats["wall_ms"] = (time.perf_counter() - t0) * 1e3
+            raise error  # only after the vote: the other ranks are waiting in it
+        return fast, slow, image
+
+    def _keep_stats(self, stats: Dict[str, float]) -> None:
         self.last_read_stats = stats
         self.passes.append(stats)
-        fut: Future = Future()
-        fut.set_result(None)
-        return fut
 
 
-class FileReader(StorageReader):
+class FileReader(_DcpReader):
     """DCP StorageReader over the files the agent wrote from the segments
     ("__<rank>_0.distcp" raw bytes + pickled ".metadata")."""
 
     def __init__(self, path: Union[str, os.PathLike]) -> None:
         super().__init__()
         self.path = Path(path)
-        self.storage_data: Dict[MetadataIndex, _StorageInfo] = {}
-        self.state_dict_metadata: Dict[str, STORAGE_TYPES] = {}
 
     def read_data(self, plan: LoadPlan, planner: LoadPlanner) -> Future[None]:
         by_file: Dict[str, List[ReadItem]] = {}
@@ -641,11 +660,7 @@ class FileReader(StorageReader):
                 for item in items:
                     info = self.storage_data[item.storage_index]
                     f.seek(info.offset)
-                    item_bytes = io.BytesIO(f.read(info.length))
-                    md = None
-                    if item.type != LoadItemType.BYTE_IO:
-                        md = self.state_dict_metadata[item.storage_index.fqn]
-                    _load_item(item, item_bytes, planner, md)
+                    self._load_stored(item, io.BytesIO(f.read(info.length)), planner)
         fut: Future = Future()
         fut.set_result(None)
         return fut
@@ -653,25 +668,6 @@ class FileReader(StorageReader):
     def read_metadata(self, *args, **kwargs) -> Metadata:
         with (self.path / ".metadata").open("rb") as f:
             return pickle.load(f)
-
-    def set_up_storage_reader(self, metadata: Metadata, is_coordinator: bool, *args,
-                              **kwargs) -> None:
-        self.storage_data = metadata.storage_data
-        self.state_dict_metadata = metadata.state_dict_metadata
-        assert self.storage_data is not None
-
-    def prepare_local_plan(self, plan: LoadPlan) -> LoadPlan:
-        return plan
-
-    def prepare_global_plan(self, global_plan: List[LoadPlan]) -> List[LoadPlan]:
-        return global_plan
-
-    def reset(self, checkpoint_id: Union[str, os.PathLike, None] = None) -> None:
-        pass
-
-    @classmethod
-    def validate_checkpoint_id(cls, checkpoint_id: Union[str, os.PathLike]) -> bool:
-        return True
 
 
 def _item_rows(md: TensorStorageMetadata, item: ReadItem, info: _StorageInfo):
@@ -747,10 +743,7 @@ class FileDmaReader(FileReader):
                 item_bytes = io.BytesIO(bytes(info.length))
                 with item_bytes.getbuffer() as view:
                     _pread_into(fds[info.relative_path], view, info.offset)
-                md = None
-                if item.type != LoadItemType.BYTE_IO:
-                    md = self.state_dict_metadata[item.storage_index.fqn]
-                _load_item(item, item_bytes, planner, md)
+                self._load_stored(item, item_bytes, planner)
             stats["read_ms"] += (time.perf_counter() - t1) * 1e3
         for item, target in targets:
             planner.commit_tensor(item, target)

@@ -1624,17 +1624,26 @@ class SharedMemoryHandler:
             raise
 
     # -- load ---------------------------------------------------------------------------
+    def _consistent_meta(self):
+        """The check every read of the in-memory checkpoint starts with: wait for this
+        handler's own drain, refuse a checkpoint that is being written, map the segment.
+        Returns (meta dict, None), or (None, why there is nothing to read)."""
+        self.wait_pending()
+        meta_dict = self.metadata.get()
+        if not meta_dict or meta_dict.get(DLROVER_CKPT_CONFIG_KEY, CheckpointConfig()).writing_shm:
+            return None, "no consistent in-memory checkpoint to restore from"
+        self.refresh_mapping()
+        if not self.shared_memory:
+            return None, "the checkpoint segment does not exist"
+        return meta_dict, None
+
     def load_state_dict(self):
         """Returns the state dict (CPU tensors aliasing the segment), or {} when
         there is no usable in-memory checkpoint."""
-        self.wait_pending()
-        meta_dict = self.metadata.get()
+        meta_dict, why = self._consistent_meta()
+        if why:
+            return {}
         config = meta_dict.get(DLROVER_CKPT_CONFIG_KEY, CheckpointConfig())
-        if not meta_dict or config.writing_shm:
-            return {}
-        self.refresh_mapping()
-        if not self.shared_memory:
-            return {}
         report_local_event(EventReportConstants.TYPE_INFO, str(config.rank),
                            EventReportConstants.ACTION_RESUME_MEM_CKPT_START,
                            f"step={config.step}")
@@ -1665,30 +1674,11 @@ class SharedMemoryHandler:
         image_first: scatter the CUDA leaves from the arena image when it covers them
         (see rollback_into); stats then carry "from_image" (1.0 / 0.0)."""
         device_ranges, host_pairs = self._restore_targets(target, strict)
-        stats = {"device_bytes": 0.0, "host_bytes": 0.0, "fill_ms": 0.0, "scatter_ms": 0.0}
-        if image_first:
-            stats["from_image"] = 0.0
         with torch.no_grad():
-            stats["host_bytes"] = self._restore_host_leaves(host_pairs)
-            if device_ranges:
-                stager, plan, stream = self._restore_plan(device_ranges, stream)
-                stats.update(self._restore_device(stager, plan, stream, image_first, coop,
-                                                  pin_after))
+            stats = {"host_bytes": self._restore_host_leaves(host_pairs)}
+            stats.update(self.read_ranges(device_ranges, stream, image_first=image_first,
+                                          coop=coop, pin_after=pin_after))
         return stats
-
-    def _restore_device(self, stager: _DeviceStager, plan, stream, image_first: bool,
-                        coop=None, pin_after: bool = True) -> Dict[str, float]:
-        """The restore of a built plan: from the arena image when image_first and it
-        covers the plan, else from the segment (cooperatively when coop is given).
-        With image_first the stats carry "from_image" (1.0 / 0.0)."""
-        got = self._run_rollback(stager, plan, stream) if image_first else None
-        if got is None and coop is not None:
-            got = self._run_restore_cooperative(stager, plan, stream, coop)
-        elif got is None:
-            got = self._run_restore(stager, plan, stream, pin_after=pin_after)
-            if image_first:
-                got["from_image"] = self.last_restore_stats["from_image"] = 0.0
-        return got
 
     def rollback_into(self, target, stream=None, strict: bool = True) -> Dict[str, float]:
         """restore_into for a process that saved the checkpoint itself: after a
@@ -1705,24 +1695,16 @@ class SharedMemoryHandler:
         """Whether rollback_into(target) would scatter every CUDA leaf from the arena
         image; restores nothing.  False when the tree has no CUDA leaf."""
         device_ranges, _ = self._restore_targets(target, strict)
-        if not device_ranges:
-            return False
-        _, plan, _ = self._restore_plan(device_ranges, None)
-        return plan.image_covers(self.shared_memory.dma_address)
+        return bool(device_ranges) and self.image_covers_ranges(device_ranges)
 
     def _restore_targets(self, target, strict: bool):
         """The part every restore of the in-memory checkpoint into live tensors shares:
-        wait for this handler's own drain, refuse a checkpoint that is being written, map
-        the segment, and pair each tensor leaf of `target` with its meta (_match_tree).
-        Returns (CUDA (tensor, segment offset, nbytes) ranges, CPU (tensor, meta) pairs)."""
-        self.wait_pending()
-        meta_dict = self.metadata.get()
-        config = meta_dict.get(DLROVER_CKPT_CONFIG_KEY, CheckpointConfig())
-        if not meta_dict or config.writing_shm:
-            raise RuntimeError("no consistent in-memory checkpoint to restore from")
-        self.refresh_mapping()
-        if not self.shared_memory:
-            raise RuntimeError("the checkpoint segment does not exist")
+        _consistent_meta (raising when there is nothing to read), then each tensor leaf of
+        `target` paired with its meta (_match_tree).  Returns (CUDA (tensor, segment
+        offset, nbytes) ranges, CPU (tensor, meta) pairs)."""
+        meta_dict, why = self._consistent_meta()
+        if why:
+            raise RuntimeError(why)
         # tuples are leaves of the memory checkpoint (plan_layout does not descend into them)
         pairs = _match_tree(target, meta_dict, TensorMeta, (list,), strict)
         device_ranges = [(t, m.offset, m.numel * m.element_size) for _, t, m in pairs if t.is_cuda]
@@ -1742,8 +1724,18 @@ class SharedMemoryHandler:
         return float(sum(m.numel * m.element_size for _, m in host_pairs))
 
     def _restore_plan(self, device_ranges, stream):
-        """(stager, restore plan, stream) for (CUDA tensor, segment offset, nbytes) ranges:
-        arena offset = segment offset, so the plan lines up with the saves' arena image."""
+        """(stager, restore plan, stream) for non-empty (CUDA tensor, segment offset,
+        nbytes) ranges, checked against the mapped segment: arena offset = segment offset,
+        so the plan lines up with the saves' arena image."""
+        self.refresh_mapping()
+        if not self.shared_memory:
+            raise RuntimeError("the checkpoint segment does not exist")
+        size = self.shared_memory.size
+        for t, off, nbytes in device_ranges:
+            if not t.is_cuda:
+                raise ValueError("read_ranges needs CUDA targets")
+            if off + nbytes > size or t.nbytes != nbytes:
+                raise ValueError("read_ranges: range does not fit the segment / the tensor")
         stager = self._stager_for([t for t, _, _ in device_ranges])
         prepared = stager.prepare_ranges(device_ranges, [], for_write=True)
         if stager._attached is None:
@@ -1814,23 +1806,32 @@ class SharedMemoryHandler:
             stager.pin_in_background()  # the next save wants plain DMA
         return dict(stats)
 
-    def read_ranges(self, device_ranges, stream=None, *,
-                    image_first: bool = False) -> Dict[str, float]:
+    def read_ranges(self, device_ranges, stream=None, *, image_first: bool = False,
+                    coop=None, pin_after: bool = True) -> Dict[str, float]:
         """Inverse of write_ranges for CUDA targets: (tensor, segment offset,
         nbytes) triples are filled by one DMA of the covered segment runs into
-        the arena + one scatter kernel into the (contiguous) tensors.
+        the arena + one scatter kernel into the (contiguous) tensors.  Every restore
+        of CUDA tensors from the in-memory checkpoint ends here.
 
         image_first: scatter from the arena image of this process's last full-snapshot
         save when it covers the ranges (one kernel, nothing crosses PCIe; see
-        rollback_into), else as above; the stats then carry "from_image" (1.0 / 0.0)."""
+        rollback_into), else as above; the stats then carry "from_image" (1.0 / 0.0).
+        coop, pin_after: see restore_into."""
         self.wait_pending()
         if not device_ranges:
             stats = {"device_bytes": 0.0, "fill_ms": 0.0, "scatter_ms": 0.0}
             if image_first:
                 stats["from_image"] = 0.0
             return stats
-        stager, plan, stream = self._read_plan(device_ranges, stream)
-        return self._restore_device(stager, plan, stream, image_first)
+        stager, plan, stream = self._restore_plan(device_ranges, stream)
+        got = self._run_rollback(stager, plan, stream) if image_first else None
+        if got is None and coop is not None:
+            got = self._run_restore_cooperative(stager, plan, stream, coop)
+        elif got is None:
+            got = self._run_restore(stager, plan, stream, pin_after=pin_after)
+            if image_first:
+                got["from_image"] = self.last_restore_stats["from_image"] = 0.0
+        return got
 
     def image_covers_ranges(self, device_ranges) -> bool:
         """Whether read_ranges(device_ranges, image_first=True) would scatter every range
@@ -1839,21 +1840,8 @@ class SharedMemoryHandler:
         self.wait_pending()
         if not device_ranges:
             return True
-        _, plan, _ = self._read_plan(device_ranges, None)
+        _, plan, _ = self._restore_plan(device_ranges, None)
         return plan.image_covers(self.shared_memory.dma_address)
-
-    def _read_plan(self, device_ranges, stream):
-        """read_ranges' checks of non-empty (CUDA tensor, segment offset, nbytes) ranges
-        against the mapped segment, then their restore plan (_restore_plan)."""
-        self.refresh_mapping()
-        if not self.shared_memory:
-            raise RuntimeError("the checkpoint segment does not exist")
-        for t, off, nbytes in device_ranges:
-            if not t.is_cuda:
-                raise ValueError("read_ranges needs CUDA targets")
-            if off + nbytes > self.shared_memory.size or t.numel() * t.element_size() != nbytes:
-                raise ValueError("read_ranges: range does not fit the segment / the tensor")
-        return self._restore_plan(device_ranges, stream)
 
     # -- queries ------------------------------------------------------------------------
     def no_checkpoint_state(self):

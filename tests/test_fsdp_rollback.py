@@ -155,6 +155,57 @@ def test_engine_rolls_back_from_the_image(cuda_device, gloo, tmp_path):
         engine.close()
 
 
+def _cpu_engine(tmp_path):
+    """An engine holding _tree("cpu") in memory at step 5, with a copy of its tensors."""
+    engine = fe.FsdpCheckpointEngine(str(tmp_path), PosixDiskStorage(), async_drain=False)
+    sd = _tree("cpu")
+    assert engine.save_to_memory(5, sd, {"model_states": str(tmp_path / "5")})
+    assert engine.wait_memory_save(60)
+    return engine, sd, {k: t.clone() for k, t in _tensors(sd).items()}
+
+
+def test_the_memory_reader_takes_no_vote(gloo, tmp_path, monkeypatch):
+    engine, sd, want = _cpu_engine(tmp_path)
+    try:
+        reader = engine.load()
+        assert type(reader) is fe.SharedMemoryReader
+
+        def collective(*args, **kwargs):
+            raise AssertionError("load()'s reader must not take part in a collective")
+
+        monkeypatch.setattr(fe, "vote_all_ranks", collective)
+        monkeypatch.setattr(fe, "all_reduce_flags", collective)
+        _scribble(sd)
+        _load(sd, reader)
+        _same(_tensors(sd), want)
+    finally:
+        engine.close()
+
+
+def test_each_rollback_pass_takes_one_vote(gloo, tmp_path, monkeypatch):
+    engine, sd, want = _cpu_engine(tmp_path)
+    votes = []
+    vote = fe.vote_all_ranks
+
+    def counted(group, check):
+        votes.append(group)
+        return vote(group, check)
+
+    monkeypatch.setattr(fe, "vote_all_ranks", counted)
+    try:
+        reader = engine.rollback_reader()
+        for n in (1, 2):  # two dcp.load passes through one reader, as rollback_checkpoint
+            _scribble(sd)
+            _load(sd, reader)
+            _same(_tensors(sd), want)
+            assert len(votes) == len(engine.last_rollback_stats()) == n
+        # CPU targets are no fast items: this rank is covered and reads nothing from HBM
+        st = reader.last_read_stats
+        assert st["fast_items"] == 0 and st["from_image"] == 1.0 and st["device_bytes"] == 0.0
+    finally:
+        engine.close()
+
+
 # ------------------------------------------------------------- a real FSDP job --
 
 

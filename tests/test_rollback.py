@@ -493,6 +493,24 @@ def test_strerror_names_the_missing_image():
     assert text and b"image" in text and text != lib.fc_strerror(-99)
 
 
+def test_a_tree_without_cuda_leaves_cannot_roll_back(run_env):
+    """CheckpointEngine.rollback_into sends such a tree to load_into."""
+    from dlrover_b200.shm_handler import DLROVER_CKPT_CONFIG_KEY, CheckpointConfig
+    from dlrover_b200.shm_handler import SharedMemoryHandler
+
+    handler = SharedMemoryHandler(0, host=True)
+    tree = {"w": torch.arange(1000, dtype=torch.float32), "step": torch.tensor(5)}
+    try:
+        handler.save_state_dict({"model_states": tree, DLROVER_CKPT_CONFIG_KEY:
+                                 CheckpointConfig(step=5, paths={"model_states": "/x/rank_0.pt"})})
+        assert handler.can_rollback({"model_states": tree}) is False
+        stats = handler.restore_into({"model_states": tree})  # the same tree does restore
+        assert stats["host_bytes"] == 4008 and stats["device_bytes"] == 0.0
+    finally:
+        handler.unlink()
+        handler.close()
+
+
 def _gloo_worker(rank, world, port, run_id, ckpt_dir, out_dir, images):
     import sys
 
